@@ -1,5 +1,5 @@
-// tests/emu/emu_lk.cpp -- the REAL bodies of the Lucas-Kanade kernels (hybvio_b200/csrc/lk.cu: CTA-per-feature hv_lk_cta_kernel<31> and
-// warp-per-feature hv_lk_kernel<31>) on the host emulator against the C oracle in the kernels' own accumulation order
+// tests/emu/emu_lk.cpp -- the REAL bodies of the Lucas-Kanade kernels (hybvio_b200/csrc/lk.cu: CTA-per-feature hv_lk_cta_kernel<WIN> and
+// warp-per-feature hv_lk_kernel<WIN>, WIN = 11, 15, 21, 31) on the host emulator against the C oracle in the kernels' own accumulation order
 // (oracle/hv_oracle_lk.c, accum_mode 1: bit-exact end points and statuses). "lk_device.inc" is the device part of lk.cu (everything
 // before the host launcher), cut out by the test that builds this file. Test infrastructure; also run under ThreadSanitizer.
 #include <algorithm>
@@ -55,28 +55,18 @@ static void to_device_layout(const orc_pyramid* p, int win, DevPyr& d)
     }
 }
 
-int main()
+template <int WIN>
+static int run_window(const std::vector<uint8_t>& a, const std::vector<uint8_t>& b, int W, int H, const std::vector<float>& prev,
+                      const std::vector<float>& init, int N)
 {
-    const int W = 320, H = 240, WIN = 31, MAXL = 3, N = 40;
-    std::vector<uint8_t> a((size_t)W * H), b((size_t)W * H);
-    for (int y = 0; y < H; y++) for (int x = 0; x < W; x++) {
-        a[(size_t)y * W + x] = (uint8_t)std::lrint(tex(x, y));
-        b[(size_t)y * W + x] = (uint8_t)std::lrint(tex(x - 2.3, y + 1.7));          // content moves by (+2.3, -1.7) px
-    }
-    for (int y = 100; y < 150; y++) for (int x = 200; x < 260; x++) a[(size_t)y * W + x] = b[(size_t)y * W + x] = 90;     // flat patch: minEig rejection
+    const int MAXL = 3;
     orc_pyramid* pa = orc_pyr_create(a.data(), W, H, W, WIN, MAXL);
     orc_pyramid* pb = orc_pyr_create(b.data(), W, H, W, WIN, MAXL);
     DevPyr da, db; to_device_layout(pa, WIN, da); to_device_layout(pb, WIN, db);
     HvPyrDesc table[2] = {da.desc, db.desc};
-    srand(7);
-    std::vector<float> prev(2 * N), init(2 * N);
-    for (int i = 0; i < N; i++) {
-        prev[2 * i] = (float)(-5 + (rand() / (double)RAND_MAX) * (W + 10)); prev[2 * i + 1] = (float)(-5 + (rand() / (double)RAND_MAX) * (H + 10));     // incl. points outside the image
-        if (i % 8 == 5) { prev[2 * i] = 230.5f; prev[2 * i + 1] = 125.25f; }                                                                          // on the flat patch
-        init[2 * i] = prev[2 * i] + 2.3f + (float)((rand() / (double)RAND_MAX) * 6 - 3); init[2 * i + 1] = prev[2 * i + 1] - 1.7f + (float)((rand() / (double)RAND_MAX) * 6 - 3);
-    }
     int fails = 0;
     for (int useInitial = 0; useInitial < 2; useInitial++) for (int variant = 0; variant < 3; variant++) {
+        if (variant == 2 && WIN != 31) continue;
         std::vector<float> onext = init, knext = init; std::vector<uint8_t> ost(N), kst(N, 7); std::vector<int32_t> kts(N, -1);
         orc_lk(pa, pb, prev.data(), onext.data(), ost.data(), N, MAXL, 20, 0.03, useInitial, 1e-3, 1);
         LkLaunch L; memset(&L, 0, sizeof(L));
@@ -85,14 +75,14 @@ int main()
         L.jobs[0].prevPts = (const float2*)prev.data(); L.jobs[0].nextPts = (float2*)knext.data(); L.jobs[0].status = kst.data(); L.jobs[0].trackStatus = kts.data();
         if (variant == 0) {
             gridDim.x = N; gridDim.y = 1;
-            for (int f = 0; f < N; f++) emu::launch_cta(LKC_NW * 32, (unsigned)f, [&] { hv_lk_cta_kernel<31>(L); });
+            for (int f = 0; f < N; f++) emu::launch_cta(LKC_NW * 32, (unsigned)f, [&] { hv_lk_cta_kernel<WIN>(L); });
         } else if (variant == 2) {                                    // 8 warps per feature (HV_LK_CTA_WARPS=8): 4 window rows per warp, the last warp owns 3
             gridDim.x = N; gridDim.y = 1;
-            for (int f = 0; f < N; f++) emu::launch_cta(8 * 32, (unsigned)f, [&] { hv_lk_cta_kernel<31, 8>(L); });
+            for (int f = 0; f < N; f++) emu::launch_cta(8 * 32, (unsigned)f, [&] { hv_lk_cta_kernel<WIN, 8>(L); });
         } else {
             const int ctas = (N + LK_WARPS_PER_CTA - 1) / LK_WARPS_PER_CTA;
             gridDim.x = ctas; gridDim.y = 1;
-            for (int c = 0; c < ctas; c++) emu::launch_cta(LK_WARPS_PER_CTA * 32, (unsigned)c, [&] { hv_lk_kernel<31>(L); });
+            for (int c = 0; c < ctas; c++) emu::launch_cta(LK_WARPS_PER_CTA * 32, (unsigned)c, [&] { hv_lk_kernel<WIN>(L); });
         }
         int bad = 0, tracked = 0;
         for (int i = 0; i < N; i++) {
@@ -100,10 +90,31 @@ int main()
             const bool same = kst[i] == ost[i] && memcmp(&knext[2 * i], &onext[2 * i], 8) == 0;
             if (!same) { bad++; if (bad < 4) printf("  feature %d: kernel (%g, %g) st %d, oracle (%g, %g) st %d\n", i, knext[2 * i], knext[2 * i + 1], kst[i], onext[2 * i], onext[2 * i + 1], ost[i]); }
         }
-        printf("%s, useInitial=%d: %d features, %d tracked, %d differ from the oracle (bit-exact end points + status)  %s\n", variant == 0 ? "hv_lk_cta_kernel<31>" : variant == 2 ? "hv_lk_cta_kernel<31, 8>" : "hv_lk_kernel<31>    ",
-               useInitial, N, tracked, bad, bad == 0 ? "ok" : "FAIL");
+        printf("%s<%d%s>, useInitial=%d: %d features, %d tracked, %d differ from the oracle (bit-exact end points + status)  %s\n",
+               variant == 1 ? "hv_lk_kernel" : "hv_lk_cta_kernel", WIN, variant == 2 ? ", 8" : "", useInitial, N, tracked, bad, bad == 0 ? "ok" : "FAIL");
         fails += bad != 0;
     }
     orc_pyr_free(pa); orc_pyr_free(pb);
     return fails;
+}
+
+int main()
+{
+    const int W = 320, H = 240, N = 40;
+    std::vector<uint8_t> a((size_t)W * H), b((size_t)W * H);
+    for (int y = 0; y < H; y++) for (int x = 0; x < W; x++) {
+        a[(size_t)y * W + x] = (uint8_t)std::lrint(tex(x, y));
+        b[(size_t)y * W + x] = (uint8_t)std::lrint(tex(x - 2.3, y + 1.7));          // content moves by (+2.3, -1.7) px
+    }
+    for (int y = 100; y < 150; y++) for (int x = 200; x < 260; x++) a[(size_t)y * W + x] = b[(size_t)y * W + x] = 90;     // flat patch: minEig rejection
+    srand(7);
+    std::vector<float> prev(2 * N), init(2 * N);
+    for (int i = 0; i < N; i++) {
+        prev[2 * i] = (float)(-5 + (rand() / (double)RAND_MAX) * (W + 10)); prev[2 * i + 1] = (float)(-5 + (rand() / (double)RAND_MAX) * (H + 10));     // incl. points outside the image
+        if (i % 8 == 5) { prev[2 * i] = 230.5f; prev[2 * i + 1] = 125.25f; }                                                                          // on the flat patch
+        init[2 * i] = prev[2 * i] + 2.3f + (float)((rand() / (double)RAND_MAX) * 6 - 3); init[2 * i + 1] = prev[2 * i + 1] - 1.7f + (float)((rand() / (double)RAND_MAX) * 6 - 3);
+    }
+    // every window size the launcher dispatches (hv_launch_lk: 11, 15, 21, 31)
+    return run_window<31>(a, b, W, H, prev, init, N) + run_window<21>(a, b, W, H, prev, init, N) + run_window<15>(a, b, W, H, prev, init, N) +
+           run_window<11>(a, b, W, H, prev, init, N);
 }

@@ -91,9 +91,9 @@ def _lk_device_part(tmp_path):
 
 
 def test_lk_kernel_bodies_on_host_emulator(tmp_path):
-    """hv_lk_cta_kernel<31> (CTA per feature, 4 and 8 warps) and hv_lk_kernel<31> (warp per feature) on the emulator: end points and statuses
-    bit-identical to the C oracle in the kernels' accumulation order, with and without initial flow, incl. points outside the image
-    and on a flat patch."""
+    """hv_lk_cta_kernel<WIN> (CTA per feature; 4 warps, and 8 at WIN = 31) and hv_lk_kernel<WIN> (warp per feature) for every window size
+    the launcher dispatches (11, 15, 21, 31) on the emulator: end points and statuses bit-identical to the C oracle in the kernels'
+    accumulation order, with and without initial flow, incl. points outside the image and on a flat patch."""
     exe = str(tmp_path / "emu_lk")
     obj = str(tmp_path / "orc_lk.o")
     incdir = _lk_device_part(tmp_path)
@@ -103,7 +103,9 @@ def test_lk_kernel_bodies_on_host_emulator(tmp_path):
                            os.path.join(ROOT, "tests", "emu", "emu_lk.cpp"), obj, "-lm", "-o", exe])
     out = subprocess.run([exe], capture_output=True, text=True, timeout=900)
     assert out.returncode == 0, out.stdout + out.stderr
-    assert out.stdout.count("  ok") == 6 and "FAIL" not in out.stdout and "35 tracked" in out.stdout and "hv_lk_cta_kernel<31, 8>" in out.stdout
+    assert out.stdout.count("  ok") == 18 and "FAIL" not in out.stdout and "hv_lk_cta_kernel<31, 8>" in out.stdout
+    for win, tracked in ((31, 35), (21, 34), (15, 33), (11, 30)):
+        assert out.stdout.count(f"<{win}") == (6 if win == 31 else 4) and f"<{win}>, useInitial=1: 40 features, {tracked} tracked" in out.stdout
 
 
 def _pyr_device_part(tmp_path):

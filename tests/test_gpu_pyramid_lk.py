@@ -120,20 +120,17 @@ def test_lk_matches_reference_golden(hv, gold):
         p.release()
 
 
-@pytest.mark.parametrize("w,h,max_level,n,use_init,seed", [
-    (752, 480, 3, 600, False, 1), (752, 480, 3, 600, True, 2), (512, 512, 3, 400, True, 3), (752, 480, 2, 100, True, 8),
-    (751, 479, 2, 200, False, 4), (100, 70, 3, 64, False, 5), (33, 40, 3, 20, True, 6), (64, 64, 0, 30, False, 7),
-    (752, 480, 3, 1000, True, 9)])   # > 640 features: warp-per-feature kernel; <= 640: CTA-per-feature kernel
-def test_lk_bit_exact_vs_oracle_exact_mode_and_close_to_reference_order(hv, oracle_lk, w, h, max_level, n, use_init, seed):
+def _lk_vs_oracle(hv, oracle_lk, w, h, max_level, use_init, seed, win, pts):
+    """LK on the GPU against the oracle: bit-exact in accum_mode 1, assert_lk_close in accum_mode 0. Returns the oracle pyramid and statuses."""
     I, _ = synth.stereo_frame(seed, w, h, seed=seed)
     J, _ = synth.stereo_frame(seed + 1, w, h, seed=seed)
     if w > 200:
         I = I.copy(); I[100:160, 100:160] = 77          # constant patch: minEig rejection
-    pts = synth.feature_points(n, w, h, seed=seed, flat_fraction=0.1 if w > 200 else 0, flat_rect=(115, 115, 145, 145))
     fx, fy = synth.true_flow(seed, seed + 1)
     init = (pts + [fx, fy] + np.random.RandomState(seed).uniform(-4, 4, pts.shape)).astype(np.float32) if use_init else None
-    pa, pb = build(hv, I, 31, max_level), build(hv, J, 31, max_level)
-    oa, ob = oracle_lk.pyramid(I, 31, max_level), oracle_lk.pyramid(J, 31, max_level)
+    pa, pb = build(hv, I, win, max_level), build(hv, J, win, max_level)
+    oa, ob = oracle_lk.pyramid(I, win, max_level), oracle_lk.pyramid(J, win, max_level)
+    assert pa.levels == oa.levels
     n_gpu, st_gpu, ts_gpu = hv.lk_track(pa, pb, pts, init)
     n1, s1, t1 = oracle_lk.lk(oa, ob, pts, init, max_level=max_level, accum_mode=1)
     assert np.array_equal(st_gpu, s1) and np.array_equal(ts_gpu, t1)
@@ -143,6 +140,105 @@ def test_lk_bit_exact_vs_oracle_exact_mode_and_close_to_reference_order(hv, orac
     assert np.array_equal(st_gpu, s0)
     assert_lk_close(n_gpu, ts_gpu, n0, t0, "vs reference-order oracle")
     pa.release(); pb.release()
+    return oa, s1
+
+
+@pytest.mark.parametrize("w,h,max_level,n,use_init,seed", [
+    (752, 480, 3, 600, False, 1), (752, 480, 3, 600, True, 2), (512, 512, 3, 400, True, 3), (752, 480, 2, 100, True, 8),
+    (751, 479, 2, 200, False, 4), (100, 70, 3, 64, False, 5), (33, 40, 3, 20, True, 6), (64, 64, 0, 30, False, 7),
+    (752, 480, 3, 1000, True, 9)])   # > 640 features: warp-per-feature kernel; <= 640: CTA-per-feature kernel
+def test_lk_bit_exact_vs_oracle_exact_mode_and_close_to_reference_order(hv, oracle_lk, w, h, max_level, n, use_init, seed):
+    pts = synth.feature_points(n, w, h, seed=seed, flat_fraction=0.1 if w > 200 else 0, flat_rect=(115, 115, 145, 145))
+    _lk_vs_oracle(hv, oracle_lk, w, h, max_level, use_init, seed, 31, pts)
+
+
+@pytest.mark.parametrize("w,h,max_level,n,use_init,seed,win", [
+    (752, 480, 5, 600, True, 11, 11), (752, 480, 5, 1000, False, 12, 11), (1280, 720, 5, 400, True, 13, 11), (96, 100, 3, 60, True, 14, 11),
+    (752, 480, 4, 500, False, 15, 15), (1280, 720, 5, 1200, True, 16, 15), (128, 140, 3, 60, False, 17, 15),
+    (752, 480, 4, 640, True, 18, 21), (1280, 720, 4, 641, False, 19, 21), (176, 200, 3, 60, True, 20, 21)])
+def test_lk_other_windows_bit_exact_vs_oracle_exact_mode_and_close_to_reference_order(hv, oracle_lk, w, h, max_level, n, use_init, seed, win):
+    """The window templates other than 31 (hv_lk_cta_kernel / hv_lk_kernel<11, 15, 21>): both kernels (n <= 640 and n > 640), 5- and
+    6-level pyramids, a coarsest level win + 1 pixels wide; uniform points (incl. the flat patch), points within `win` of every border and
+    far-out points."""
+    pts = synth.feature_points(n, w, h, seed=seed, flat_fraction=0.1 if w > 200 else 0, flat_rect=(115, 115, 145, 145))
+    rng = np.random.RandomState(seed)
+    k = 8
+    xs = np.concatenate([rng.uniform(0, win, k), rng.uniform(w - win, w, k), rng.uniform(0, w, 2 * k)])
+    ys = np.concatenate([rng.uniform(0, h, 2 * k), rng.uniform(0, win, k), rng.uniform(h - win, h, k)])
+    far = [[-3 * win, h / 2], [w + 3 * win, h / 2], [w / 2, -1e4], [1e6, 1e6]]
+    pts = np.concatenate([pts[:n - len(xs) - len(far)], np.stack([xs, ys], 1), far]).astype(np.float32)
+    oa, s1 = _lk_vs_oracle(hv, oracle_lk, w, h, max_level, use_init, seed, win, pts)
+    if w < 200:
+        assert oa.level_size(oa.levels - 1)[0] == win + 1
+    assert 0 < s1.sum() < len(s1)                      # the flat patch and far-out points fail, the rest track
+
+
+@pytest.mark.parametrize("max_iter,eps,min_eig", [(m, 0.03, 1e-3) for m in (0, 1, 5, 100, 150)] +
+                         [(20, e, 1e-3) for e in (0.0, 1e-6, 0.5, 20.0)] + [(20, 0.03, me) for me in (0.0, 1e-2)])
+def test_lk_termination_criteria_bit_exact_vs_oracle(hv, oracle_lk, max_iter, eps, min_eig):
+    """Other max_iter / eps / min_eig than the tracker's defaults, incl. values the criteria clamp (max_iter <= 100, eps <= 10) limits."""
+    I, _ = synth.stereo_frame(40, 752, 480, seed=40)
+    J, _ = synth.stereo_frame(41, 752, 480, seed=40)
+    I = I.copy(); I[100:160, 100:160] = 77
+    pts = synth.feature_points(300, 752, 480, seed=40, flat_fraction=0.1, flat_rect=(115, 115, 145, 145))
+    pa, pb = build(hv, I), build(hv, J)
+    oa, ob = oracle_lk.pyramid(I), oracle_lk.pyramid(J)
+    n_gpu, st_gpu, ts_gpu = hv.lk_track(pa, pb, pts, None, max_iter=max_iter, eps=eps, min_eig=min_eig)
+    n1, s1, t1 = oracle_lk.lk(oa, ob, pts, None, max_iter=max_iter, eps=eps, min_eig=min_eig, accum_mode=1)
+    assert np.array_equal(st_gpu, s1) and np.array_equal(ts_gpu, t1)
+    assert np.array_equal(n_gpu.view(np.uint32), n1.view(np.uint32)), np.abs(n_gpu - n1).max()
+    pa.release(); pb.release()
+
+
+def test_lk_batch_device_matches_single_jobs(hv):
+    """hv_lk_track_batch_device: jobs of unequal n (incl. 0), 11 jobs (two launches of at most 8), totals above 640 with every job below
+    it (the kernel is picked on the total): every job equals the same job issued alone through hv_lk_track_device, bit for bit; mixed
+    window sizes are rejected."""
+    import torch
+    from hybvio_b200 import capi
+    frames = [synth.stereo_frame(50 + k)[0] for k in range(4)]
+    pyrs = [build(hv, f) for f in frames]
+
+    def job_set(sizes):
+        out = []
+        for i, n in enumerate(sizes):
+            pts = synth.feature_points(max(n, 1), seed=60 + i)[:n]
+            out.append((pyrs[i % 3], pyrs[i % 3 + 1], torch.from_numpy(np.ascontiguousarray(pts)).cuda().reshape(n, 2), n))
+        return out
+
+    def run_batch(js):
+        res = [(torch.full((n, 2), -1.0, device="cuda"), torch.zeros(n, dtype=torch.uint8, device="cuda"),
+                torch.full((n,), -1, dtype=torch.int32, device="cuda")) for _, _, _, n in js]
+        jobs = (capi.LkJob * len(js))()
+        for k, ((a, b, d, n), (nx, st, ts)) in enumerate(zip(js, res)):
+            jobs[k].prev, jobs[k].next, jobs[k].n, jobs[k].use_initial = a.h, b.h, n, 0
+            jobs[k].d_prev_xy, jobs[k].d_next_xy, jobs[k].d_status, jobs[k].d_track_status = d.data_ptr(), nx.data_ptr(), st.data_ptr(), ts.data_ptr()
+        torch.cuda.synchronize()
+        capi.check(hv.lib.hv_lk_track_batch_device(hv.h, jobs, len(js), 20, 0.03, 1e-3), "hv_lk_track_batch_device")
+        hv.sync()
+        return [tuple(x.cpu().numpy() for x in r) for r in res]
+
+    for sizes in ([150, 0, 37, 300, 1], [100, 90, 80, 70, 60, 50, 40, 30, 20, 10, 5], [600, 500, 100]):
+        js = job_set(sizes)
+        got = run_batch(js)
+        for (a, b, d, n), (nx, st, ts) in zip(js, got):
+            if n == 0:
+                continue
+            nx1 = torch.zeros((n, 2), device="cuda"); st1 = torch.zeros(n, dtype=torch.uint8, device="cuda"); ts1 = torch.zeros(n, dtype=torch.int32, device="cuda")
+            hv.lk_track_device(a, b, d, nx1, st1, ts1, n, False)
+            hv.sync()
+            assert np.array_equal(nx.view(np.uint32), nx1.cpu().numpy().view(np.uint32)), sizes
+            assert np.array_equal(st, st1.cpu().numpy()) and np.array_equal(ts, ts1.cpu().numpy()), sizes
+    p11a, p11b = build(hv, frames[0], 11), build(hv, frames[1], 11)
+    d = torch.from_numpy(synth.interior_points(10)).cuda()
+    out = [torch.zeros((10, 2), device="cuda"), torch.zeros(10, dtype=torch.uint8, device="cuda"), torch.zeros(10, dtype=torch.int32, device="cuda")]
+    jobs = (capi.LkJob * 2)()
+    for k, (a, b) in enumerate(((pyrs[0], pyrs[1]), (p11a, p11b))):
+        jobs[k].prev, jobs[k].next, jobs[k].n, jobs[k].use_initial = a.h, b.h, 10, 0
+        jobs[k].d_prev_xy, jobs[k].d_next_xy, jobs[k].d_status, jobs[k].d_track_status = d.data_ptr(), out[0].data_ptr(), out[1].data_ptr(), out[2].data_ptr()
+    assert hv.lib.hv_lk_track_batch_device(hv.h, jobs, 2, 20, 0.03, 1e-3) == -1          # HV_ERR_INVALID
+    for p in pyrs + [p11a, p11b]:
+        p.release()
 
 
 def test_lk_edge_cases(hv):

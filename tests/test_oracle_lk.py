@@ -88,16 +88,13 @@ def test_oracle_exact_integer_mode_is_within_tolerance_of_reference_order(oracle
     assert (d > 1e-3).sum() <= -(-d.size // 1000) and d.max() < 3e-2
 
 
-@pytest.mark.parametrize("w,h,max_level,n,use_init,seed", [
-    (752, 480, 3, 400, False, 1), (752, 480, 3, 400, True, 2), (512, 512, 3, 300, True, 3),
-    (751, 479, 2, 200, False, 4), (100, 70, 3, 50, False, 5), (33, 40, 3, 20, True, 6), (64, 64, 0, 30, False, 7)])
-def test_oracle_bit_exact_vs_compiled_reference(oracle_lk, ref_lk, w, h, max_level, n, use_init, seed):
+def _oracle_vs_reference(oracle_lk, ref_lk, w, h, max_level, n, use_init, seed, win):
     I, _ = synth.stereo_frame(seed, w, h, seed=seed)
     J, _ = synth.stereo_frame(seed + 1, w, h, seed=seed)
     if w > 200:
         I = I.copy(); I[100:160, 100:160] = 77
-    ra, rb = ref_lk.pyramid(I, 31, max_level), ref_lk.pyramid(J, 31, max_level)
-    oa, ob = oracle_lk.pyramid(I, 31, max_level), oracle_lk.pyramid(J, 31, max_level)
+    ra, rb = ref_lk.pyramid(I, win, max_level), ref_lk.pyramid(J, win, max_level)
+    oa, ob = oracle_lk.pyramid(I, win, max_level), oracle_lk.pyramid(J, win, max_level)
     assert ra.levels == oa.levels
     for lv in range(ra.levels):
         for x, y in zip(ra.download(lv), oa.download(lv)):
@@ -109,6 +106,20 @@ def test_oracle_bit_exact_vs_compiled_reference(oracle_lk, ref_lk, w, h, max_lev
     n2, s2, t2 = oracle_lk.lk(oa, ob, pts, init, max_level=max_level, accum_mode=0)
     assert np.array_equal(s1, s2) and np.array_equal(t1, t2)
     assert np.array_equal(n1.view(np.uint32), n2.view(np.uint32))
+
+
+@pytest.mark.parametrize("w,h,max_level,n,use_init,seed", [
+    (752, 480, 3, 400, False, 1), (752, 480, 3, 400, True, 2), (512, 512, 3, 300, True, 3),
+    (751, 479, 2, 200, False, 4), (100, 70, 3, 50, False, 5), (33, 40, 3, 20, True, 6), (64, 64, 0, 30, False, 7)])
+def test_oracle_bit_exact_vs_compiled_reference(oracle_lk, ref_lk, w, h, max_level, n, use_init, seed):
+    _oracle_vs_reference(oracle_lk, ref_lk, w, h, max_level, n, use_init, seed, 31)
+
+
+@pytest.mark.parametrize("w,h,max_level,n,use_init,seed,win", [
+    (752, 480, 5, 400, True, 11, 11), (96, 100, 3, 50, False, 14, 11), (752, 480, 4, 300, False, 15, 15), (1280, 720, 4, 300, True, 19, 21)])
+def test_oracle_other_windows_bit_exact_vs_compiled_reference(oracle_lk, ref_lk, w, h, max_level, n, use_init, seed, win):
+    """pyrLKWindowSize 11, 15, 21 (the reference's LK is compiled for any window; the oracle restates it)."""
+    _oracle_vs_reference(oracle_lk, ref_lk, w, h, max_level, n, use_init, seed, win)
 
 
 def test_oracle_empty_and_single_point(oracle_lk):
