@@ -69,13 +69,16 @@ __device__ __forceinline__ int unaug_src(int i, int poseTrailDim)
     return -1;
 }
 
+// sym: a deferred maintainPositiveSemiDefinite() is applied while P is read (the operand pair of symmetrize())
 template <class SrcFn>
-__device__ __forceinline__ void shift_state(const double* __restrict__ P, double* __restrict__ P2, double* m, int N, SrcFn src)
+__device__ __forceinline__ void shift_state(const double* __restrict__ P, double* __restrict__ P2, double* m, int N, SrcFn src, bool sym = false)
 {
     for (int idx = blockIdx.x * blockDim.x + threadIdx.x; idx < N * N; idx += gridDim.x * blockDim.x) {
         const int i = idx % N, j = idx / N;
         const int si = src(i), sj = src(j);
-        P2[idx] = (si < 0 || sj < 0) ? 0.0 : P[si + (size_t)sj * N];
+        double v = (si < 0 || sj < 0) ? 0.0 : P[si + (size_t)sj * N];
+        if (sym && si >= 0 && sj >= 0 && si != sj) v = 0.5 * (v + P[sj + (size_t)si * N]);
+        P2[idx] = v;
     }
     if (blockIdx.x != 0) return;   // the state vector is shifted by block 0
     double tmp[4];   // N <= 4 * EKF_NT
@@ -106,7 +109,7 @@ __global__ void __launch_bounds__(EKF_NT) ekf_update_kernel(EkfUpdateArgs a)
     // ---- phase 0 (augmentation only): m = A m, P = A P A' + visAugQ  (ekf.cpp:853-857), out of place into P2
     if (a.op == EKF_OP_AUGMENT) {
         const int drop = a.dropIdx;
-        shift_state(P, a.b.P2, m, N, [drop](int i) { return aug_src(i, drop); });
+        shift_state(P, a.b.P2, m, N, [drop](int i) { return aug_src(i, drop); }, a.symFirst != 0);
         __syncthreads();
         P = a.b.P2;
         if (tid < EKF_POSE) P[(EKF_CAM + tid) * (size_t)(N + 1)] += tid < 3 ? a.augNoisePos : a.augNoiseOri;
@@ -171,10 +174,10 @@ __global__ void __launch_bounds__(EKF_NT) ekf_update_kernel(EkfUpdateArgs a)
             s_scalar[0] = sqrt(ss / n);
         }
         __syncthreads();
-        if (s_scalar[0] > a.rmseThr) { if (tid == 0) { a.b.res[0] = 2.0; a.b.res[1] = 0.0; a.b.res[2] = 0.0; } return; }
+        if (s_scalar[0] > a.rmseThr) { if (tid == 0) ekf_report(a, 2.0, 0.0, 0.0); return; }
     }
     if (checking && a.skipChi2 && a.mode == EKF_MODE_CHECK) {   // ekf.cpp:803
-        if (tid == 0) { a.b.res[0] = 0.0; a.b.res[1] = 0.0; a.b.res[2] = 0.0; }
+        if (tid == 0) ekf_report(a, 0.0, 0.0, 0.0);
         return;
     }
 
@@ -227,7 +230,7 @@ __global__ void __launch_bounds__(EKF_NT) ekf_update_kernel(EkfUpdateArgs a)
         }
         __syncthreads();
     }
-    if (bad) { if (tid == 0) { a.b.res[0] = 1.0 /*NOT_COMPUTED*/; a.b.res[1] = 0.0; a.b.res[2] = 1.0; } return; }
+    if (bad) { if (tid == 0) ekf_report(a, 1.0 /*NOT_COMPUTED*/, 0.0, 1.0); return; }
 
     // ---- phase 5: scale row k by d_k^-1/2 (Z = D^-1/2 L^-1 [HP | v]); chi2 = noiseScale |z_v|^2 (ekf.cpp:815)
     for (int k = wrp; k < n; k += nwarps) {
@@ -244,9 +247,9 @@ __global__ void __launch_bounds__(EKF_NT) ekf_update_kernel(EkfUpdateArgs a)
     const double chi2 = s_scalar[1];
     if (checking) {
         const bool outlier = !a.skipChi2 && chi2 > a.chi2Thr;
-        if (tid == 0) { a.b.res[0] = outlier ? 3.0 : 0.0; a.b.res[1] = chi2; a.b.res[2] = 0.0; }
+        if (tid == 0) ekf_report(a, outlier ? 3.0 : 0.0, chi2, 0.0);
         if (outlier || a.mode == EKF_MODE_CHECK) return;
-    } else if (tid == 0) { a.b.res[0] = 0.0; a.b.res[1] = chi2; a.b.res[2] = 0.0; }
+    } else if (tid == 0) ekf_report(a, 0.0, chi2, 0.0);
 
     // ---- phase 6: m += Z' z_v;  P -= Z' Z  (lower 4x4 blocks, mirrored)
     for (int i = tid; i < N; i += EKF_NT) {
@@ -525,29 +528,31 @@ __global__ void __launch_bounds__(EKF_NT) ekf_ew_heavy_kernel(EkfEwArgs a)
 }
 
 // ------------------------------------------------------------------------------------------------ launch
-size_t ekf_update_smem_bytes(int n, int N) { return (size_t)n * (size_t)((n + N + 1) | 1) * sizeof(double); }
+static size_t ekf_update_smem_bytes(int n, int N) { return (size_t)n * (size_t)((n + N + 1) | 1) * sizeof(double); }
 static size_t ekf_augment_smem_bytes(int N)
 {
     const int n = EKF_POSE;
     return ((size_t)n * (size_t)((n + N + 1 + n) | 1) + (size_t)N * 21) * sizeof(double);
 }
 
-bool ekf_update_uses_cluster2(const EkfUpdateArgs& a)
-{
-    return !a.useGlobalWork && ekf_cluster2_fits(a.n, a.l, a.b.N, a.op == EKF_OP_AUGMENT);
-}
-
-cudaError_t ekf_launch_update(const EkfUpdateArgs& a, cudaStream_t s)
+cudaError_t ekf_launch_update(const EkfUpdateArgs& args, cudaStream_t s)
 {
     // 8-CTA cluster kernel (ekf_cluster2.cuh) whenever its shared-memory working set fits (n <= 84 at N = 160); the single-CTA
-    // kernel below only for oversized measurements (batch updates with n up to N, tableau in global memory).
-    if (ekf_update_uses_cluster2(a)) return ekf_launch_update_cluster2(a, s);
+    // kernel below only for oversized measurements (batch updates with n up to N, tableau in global memory above 200 KB).
+    if (ekf_cluster2_fits(args.n, args.l, args.b.N, args.op == EKF_OP_AUGMENT)) return ekf_launch_update_cluster2(args, s);
     static bool seen[64];                             // per device: function attributes belong to the device's context
     if (hv_first_use_on_device(seen)) {
         cudaError_t e = cudaFuncSetAttribute(ekf_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
         if (e != cudaSuccess) return e;
     }
-    const size_t smem = a.op == EKF_OP_AUGMENT ? ekf_augment_smem_bytes(a.b.N) : a.useGlobalWork ? 0 : ekf_update_smem_bytes(a.n, a.b.N);
+    EkfUpdateArgs a = args;
+    size_t smem;
+    if (a.op == EKF_OP_AUGMENT) { a.useGlobalWork = 0; smem = ekf_augment_smem_bytes(a.b.N); }
+    else {
+        smem = ekf_update_smem_bytes(a.n, a.b.N);
+        a.useGlobalWork = smem > 200 * 1024 ? 1 : 0;
+        if (a.useGlobalWork) smem = 0;
+    }
     ekf_update_kernel<<<1, EKF_NT, smem, s>>>(a);
     return cudaGetLastError();
 }

@@ -30,7 +30,7 @@ struct EkfBufs {
     double* P;        // N x N   (current)
     double* P2;       // N x N   (target of out-of-place shifts/transforms; host swaps after the launch)
     double* work;     // global fallback for the elimination tableau when it does not fit shared memory
-    double* cwork;    // cluster kernel exchange buffers through L2: 8 partial S | reduced S | gathered Z  (10 x N x N)
+    double* cwork;    // cluster kernel exchange buffers through L2: gathered Z | reduced S | 8 partial S  (10 x N x N)
     double* Hs;       // EKF_SMALL_MAXN x EKF_SMALL_MAXL built-in measurement matrix
     double* Q;        // 12 x 12 process noise
     double* dydx;     // 20 x 20 last predict Jacobian (getDydx)
@@ -74,18 +74,18 @@ struct EkfUpdateArgs {
     int dropIdx;          // EKF_OP_AUGMENT: discarded pose index
     double augNoisePos, augNoiseOri;   // visAugQ diagonal (noiseScale applied)
     double defaultSpeed;  // EKF_OP_PSEUDO_VELOCITY
-    int useGlobalWork;    // tableau in b.work instead of shared memory
-    int symFirst;         // EKF_OP_AUGMENT (cluster kernel): a deferred maintainPositiveSemiDefinite() is applied while P is read
-    // Result words for a polling host (ekf_cluster2.cuh only): sig[0..2] = res[0..2], then sig[3] = sigSeq, written to
+    int useGlobalWork;    // tableau in b.work instead of shared memory (set by ekf_launch_update)
+    int symFirst;         // EKF_OP_AUGMENT: a deferred maintainPositiveSemiDefinite() is applied while P is read
+    // Result words for a polling host (both update kernels, ekf_report): sig[0..2] = res[0..2], then sig[3] = sigSeq, written to
     // mapped pinned host memory at decision time (a check+update continues with the update afterwards). NULL: none.
     double* sig;
     double sigSeq;
     // Device-side control flow (ekf_cluster2.cuh only) for chains that are issued without host round trips
     // (hv_ekf_visual_tracks): the kernel does its work only if
     //   (gateI == NULL || *gateI == gateIExpect) && (gateD == NULL || *gateD == gateDExpect) && (counter == NULL || *counter < counterMax),
-    // otherwise it reports NOT_COMPUTED and leaves the filter alone. slot (3 doubles, device) receives the result words as well;
-    // *bump is incremented once an update has been applied. lateH: the measurement model is produced by the preceding kernel
-    // of the stream, so it may only be read after griddepcontrol.wait.
+    // otherwise it reports NOT_COMPUTED and leaves the filter alone. slot (3 doubles, device; both update kernels) receives the
+    // result words as well; *bump is incremented once an update has been applied. lateH: the measurement model is produced by
+    // the preceding kernel of the stream, so it may only be read after griddepcontrol.wait.
     const int* gateI; int gateIExpect;
     const double* gateD; double gateDExpect;
     const int* counter; int counterMax;
@@ -102,6 +102,19 @@ struct EkfUpdateArgs {
     // backend.cpp:1158-1185, in one kernel: H P and S0 = H P H' are formed once, S0 + R is factorised twice.
     double Rdiag2;
 };
+
+// Result words (VuOutlierStatus, chi2, numeric flag), written by one thread of an update kernel at each decision: device copy,
+// optional device slot, optional mapped-host copy whose sequence word follows the other three
+__device__ __forceinline__ void ekf_report(const EkfUpdateArgs& a, double st, double chi2, double flag)
+{
+    a.b.res[0] = st; a.b.res[1] = chi2; a.b.res[2] = flag;
+    if (a.slot) { a.slot[0] = st; a.slot[1] = chi2; a.slot[2] = flag; }
+    if (a.sig) {
+        a.sig[0] = st; a.sig[1] = chi2; a.sig[2] = flag;
+        __threadfence_system();
+        ((volatile double*)a.sig)[3] = a.sigSeq;
+    }
+}
 
 // Independent outlier checks against the same (m, P): one launch, one 8-CTA cluster per measurement
 #define EKF_MAX_BATCH 24
@@ -150,10 +163,9 @@ struct EkfEwArgs {
     double dval[8];
 };
 
-size_t ekf_update_smem_bytes(int n, int N);
 cudaError_t ekf_launch_update(const EkfUpdateArgs& a, cudaStream_t s);
+// ekf_launch_update picks the cluster kernel (the only one with specP / specM, Rdiag2 and the device-side gates) iff this holds
 bool ekf_cluster2_fits(int n, int l, int N, bool joseph);
-bool ekf_update_uses_cluster2(const EkfUpdateArgs& a);    // the kernel ekf_launch_update will pick reports through a.sig
 cudaError_t ekf_launch_update_cluster2(const EkfUpdateArgs& a, cudaStream_t s);
 // aug != NULL: one more cluster of the same launch runs the augmentation *aug (results into aug->specP / aug->specM)
 cudaError_t ekf_launch_check_batch2(const EkfUpdateArgs& a, const EkfCheckBatch& b, cudaStream_t s, const EkfUpdateArgs* aug = nullptr);

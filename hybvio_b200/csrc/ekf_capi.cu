@@ -144,17 +144,11 @@ extern "C" { static int staging_acquire(hv_ekf* e); }
 #define EKF_ENTER(e, who)                              \
     do { EKF_ENTER_LAZY(e, who); int rc2_ = flush_pending(e); if (rc2_ != HV_OK) return rc2_; } while (0)
 
-static void prep_update(hv_ekf* e, EkfUpdateArgs& a)
-{
-    a.b = e->b;
-    a.noiseScale = e->noiseScale;
-    const size_t need = ekf_update_smem_bytes(a.n, e->N);
-    a.useGlobalWork = (a.op != EKF_OP_AUGMENT && need > 200 * 1024 && !ekf_cluster2_fits(a.n, a.l, e->N, false)) ? 1 : 0;
-}
 static int launch_update(hv_ekf* e, EkfUpdateArgs& a)
 {
     e->epoch++;
-    prep_update(e, a);
+    a.b = e->b;
+    a.noiseScale = e->noiseScale;
     HV_CUDA(ekf_launch_update(a, e->ctx->stream));
     e->ctx->launches++;
     return HV_OK;
@@ -673,7 +667,7 @@ static int staging_release(hv_ekf* e)      // call right after the H2D copy has 
     return HV_OK;
 }
 
-// Waits for `count` result slots of the mapped buffer to carry sequence number seq (kernels of ekf_cluster2.cuh).
+// Waits for `count` result slots of the mapped buffer to carry sequence number seq (written by ekf_report).
 static int poll_results(hv_ekf* e, int count, double seq, const char* who)
 {
     cudaStream_t s = e->ctx->stream;
@@ -728,12 +722,13 @@ static int visual_host(hv_ekf* e, const char* who, const double* H, int n, int l
     rc = staging_release(e);
     if (rc != HV_OK) return rc;
     a.H = e->d_in; a.f = e->d_in + nl; a.y = e->d_in + nl + n;
-    prep_update(e, a);
-    const bool polled = ekf_polling() && mode != EKF_MODE_UPDATE && !mOut && ekf_update_uses_cluster2(a);
+    const bool polled = ekf_polling() && mode != EKF_MODE_UPDATE && !mOut;
     if (polled) { a.sig = e->d_sig; a.sigSeq = (e->sigSeq += 1.0); }
     // A pure check speculates: the same kernel goes on to compute the update the reference issues for an INLIER (with the noise level of the
-    // previous updateVisualTrack) into P2 / m2, while the host already has the decision; P and m stay as they are.
-    const bool speculate = polled && mode == EKF_MODE_CHECK && e->specEnabled && e->specR > 0.0 && !a.skipChi2 && a.rmseThr < 0.0 && r > 0.0;
+    // previous updateVisualTrack) into P2 / m2, while the host already has the decision; P and m stay as they are. Only the cluster kernel
+    // has the second buffers (the single-CTA kernel would update P in place).
+    const bool speculate = polled && mode == EKF_MODE_CHECK && e->specEnabled && e->specR > 0.0 && !a.skipChi2 && a.rmseThr < 0.0 && r > 0.0 &&
+                           ekf_cluster2_fits(n, l, e->N, false);
     if (speculate) {
         int rcj = join_side(e);
         if (rcj != HV_OK) return rcj;
@@ -796,13 +791,10 @@ static int visual_device(hv_ekf* e, const double* dH, int n, int l, const double
     // caller-owned device pointers: H may have been produced by the caller's previous kernel on this stream (hv_ctx_create_on_stream),
     // so it is staged AFTER griddepcontrol.wait; early staging is kept for H that arrived through the library's own H2D copy
     a.lateH = lateH;
-    prep_update(e, a);
-    const bool ownSlot = slot && ekf_update_uses_cluster2(a);      // the cluster kernel writes its result words into the slot itself
-    if (ownSlot) a.slot = slot;
+    a.slot = slot;                                                 // the kernel writes its result words into the slot itself
     rc = launch_update(e, a);
     if (rc != HV_OK) return rc;
     if (dResult) HV_CUDA(cudaMemcpyAsync(dResult, e->b.res, 2 * sizeof(double), cudaMemcpyDeviceToDevice, e->ctx->stream));
-    if (slot && !ownSlot) HV_CUDA(cudaMemcpyAsync(slot, e->b.res, 3 * sizeof(double), cudaMemcpyDeviceToDevice, e->ctx->stream));
     return HV_OK;
 }
 
@@ -839,15 +831,9 @@ int hv_ekf_augment(hv_ekf* e, int discarded)
     if (rcf != HV_OK) return rcf;
     if (discarded == -1) discarded = e->trail - 1;               // ekf.cpp:849
     if (discarded < 0 || discarded >= e->trail) { hv_set_error("hv_ekf_augment: pose index %d out of range", discarded); return HV_ERR_INVALID; }
-    EkfUpdateArgs a; augment_args(e, discarded, false, a);
-    if (!ekf_update_uses_cluster2(a)) { int rcj = join_side(e); if (rcj != HV_OK) return rcj; }      // the single-CTA kernel shifts into P2
-    if (ekf_update_uses_cluster2(a)) {                           // a deferred symmetrisation rides along (cluster kernel only)
-        a.symFirst = e->pendSym ? 1 : 0;
-        e->pendSym = false;
-    } else {                                                     // the single-CTA kernel has no fused variant: issue it first
-        int rcs = flush_sym(e);
-        if (rcs != HV_OK) return rcs;
-    }
+    EkfUpdateArgs a; augment_args(e, discarded, e->pendSym, a);  // a deferred symmetrisation rides along
+    e->pendSym = false;
+    if (!ekf_cluster2_fits(a.n, a.l, e->N, true)) { int rcj = join_side(e); if (rcj != HV_OK) return rcj; }      // the single-CTA kernel shifts into P2
     int rc = launch_update(e, a);   // shift into P2, update there, Joseph product back into P: no swap
     if (rc != HV_OK) return rc;
     augment_done(e);
@@ -968,7 +954,7 @@ static int flush_checks(hv_ekf* e, const hv_ekf_op* ops, int first, int count, b
         int rc = staging_release(e);
         if (rc != HV_OK) return rc;
     }
-    a.b = e->b; a.noiseScale = e->noiseScale; a.useGlobalWork = 0;
+    a.b = e->b; a.noiseScale = e->noiseScale;
     const bool polled = host && ekf_polling();           // every item fits the cluster kernel (batchable_check)
     if (polled) { a.sig = e->d_sig; a.sigSeq = (e->sigSeq += 1.0); }
     if (!host && first + count <= HV_RUN_MAX_OPS) a.slot = e->d_opres + 4 * first;      // hv_ekf_run_device_results
@@ -998,7 +984,6 @@ static int flush_checks(hv_ekf* e, const hv_ekf_op* ops, int first, int count, b
             HV_CUDA(cudaEventRecord(e->evJoin, side));
             e->sideBusy = true;
             e->ctx->launches++;
-            aug.useGlobalWork = 0;
             HV_CUDA(ekf_launch_update(aug, s));
         }
         adopt_second_buffers(e);
@@ -1078,7 +1063,7 @@ static int run_ops(hv_ekf* e, const hv_ekf_op* ops, int nops, bool host, int* vu
 // its update is applied, so nothing the host would do depends on an intermediate result. Every measurement gets its own slice of the
 // pinned staging block (the host stages and issues op i+1 while the GPU works on op i), the kernels write their result words into a
 // mapped pinned area (one 4-double slot per op), and the ONE synchronisation at the end also covers the state read-back.
-// Returns 1 if the list cannot be handled here (too long, staging too small, a measurement that needs the single-CTA kernel).
+// Leaves *handled = 0 if the list cannot be handled here (too long, staging too small, an invalid visual op: run_ops reports it).
 static int run_ops_host_async(hv_ekf* e, const hv_ekf_op* ops, int nops, int* vuStatus, double* chi2, double* mOut, int* handled)
 {
     *handled = 0;
@@ -1087,7 +1072,7 @@ static int run_ops_host_async(hv_ekf* e, const hv_ekf_op* ops, int nops, int* vu
     for (int i = 0; i < nops; i++) {
         const hv_ekf_op& o = ops[i];
         if (o.kind != HV_EKF_OP_VISUAL) continue;
-        if (o.mode < 0 || o.mode > 2 || !o.H || !o.f || !o.y || o.n <= 0 || o.l <= 0 || o.l > e->N || o.n > e->N || !ekf_cluster2_fits(o.n, o.l, e->N, false)) return HV_OK;
+        if (o.mode < 0 || o.mode > 2 || !o.H || !o.f || !o.y || o.n <= 0 || o.l <= 0 || o.l > e->N || o.n > e->N) return HV_OK;
         need += (size_t)o.n * o.l + 2 * (size_t)o.n;
     }
     if (need > e->inDoubles) return HV_OK;
@@ -1111,9 +1096,10 @@ static int run_ops_host_async(hv_ekf* e, const hv_ekf_op* ops, int nops, int* vu
         if (o.kind == HV_EKF_OP_VISUAL) {
             rc = flush_pending(e);
             if (rc != HV_OK) return rc;
-            // consecutive pure checks: one launch (one cluster per track)
+            // consecutive pure checks that fit the cluster kernel: one launch (one cluster per track)
+            const bool batch = batchable_check(e, o);
             int cnt = 1;
-            if (o.mode == EKF_MODE_CHECK) while (i + cnt < nops && cnt < EKF_MAX_BATCH && ops[i + cnt].kind == HV_EKF_OP_VISUAL && ops[i + cnt].mode == EKF_MODE_CHECK) cnt++;
+            if (batch) while (i + cnt < nops && cnt < EKF_MAX_BATCH && batchable_check(e, ops[i + cnt])) cnt++;
             EkfUpdateArgs a; EkfCheckBatch b;
             memset(&b, 0, sizeof(b));
             b.count = cnt;
@@ -1152,9 +1138,9 @@ static int run_ops_host_async(hv_ekf* e, const hv_ekf_op* ops, int nops, int* vu
             group++;
             a.sig = e->d_run + 4 * i; a.sigSeq = seq;
             int disc = -1; bool sym = false;
-            const int extra = o.mode == EKF_MODE_CHECK ? augment_follows(e, ops, nops, i + cnt, &disc, &sym) : 0;
+            const int extra = batch ? augment_follows(e, ops, nops, i + cnt, &disc, &sym) : 0;
             if (cnt > 1 || extra) {
-                a.b = e->b; a.noiseScale = e->noiseScale; a.useGlobalWork = 0;
+                a.b = e->b; a.noiseScale = e->noiseScale;
                 if (extra) {
                     rc = join_side(e);
                     if (rc != HV_OK) return rc;
@@ -1450,8 +1436,7 @@ int hv_ekf_visual_tracks(hv_ekf* e, const hv_track_obs* tracks, int ntracks, con
             c.H = t->d_H + (size_t)k * TrackModels::hStride(); c.f = t->d_f + (size_t)k * 2 * TM_MAXOBS; c.y = base.ip + (size_t)k * 2 * TM_MAXOBS;
             c.gateI = base.status + 4 * (size_t)k + 1; c.gateIExpect = 0; c.counter = d_counter; c.counterMax = maxSucc; c.slot = slotC; c.lateH = 1;
             if (fused) { c.Rdiag2 = (p->visual_r * p->visual_r) * e->noiseScale; c.bump = d_counter; }      // check with chi_outlier_r, update with visual_r, one kernel
-            prep_update(e, c);
-            if (!ekf_update_uses_cluster2(c)) { hv_set_error("%s: track %d (n=%d, l=%d) does not fit the cluster kernel", who, k, n, l); return HV_ERR_INVALID; }
+            if (!ekf_cluster2_fits(n, l, e->N, false)) { hv_set_error("%s: track %d (n=%d, l=%d) does not fit the cluster kernel", who, k, n, l); return HV_ERR_INVALID; }
             rc = launch_update(e, c);
             if (rc != HV_OK) return rc;
             if (fused) continue;
@@ -1505,8 +1490,7 @@ int hv_ekf_visual_track(hv_ekf* e, const hv_track_model* t, double r, double rms
     int rc = visual_args(e, who, t->rows, t->cols, r, rmseThr, mode, a);
     if (rc != HV_OK) return rc;
     a.H = t->d_H; a.f = t->d_f; a.y = t->d_y;
-    prep_update(e, a);
-    const bool polled = ekf_polling() && mode != EKF_MODE_UPDATE && ekf_update_uses_cluster2(a);
+    const bool polled = ekf_polling() && mode != EKF_MODE_UPDATE;
     if (polled) { a.sig = e->d_sig; a.sigSeq = (e->sigSeq += 1.0); }
     rc = launch_update(e, a);
     if (rc != HV_OK) return rc;

@@ -1,5 +1,5 @@
 // hybvio_b200/csrc/ekf_cluster2.cu -- kernels and launchers of the second-generation cluster update (ekf_cluster2.cuh):
-// P column blocks resident in shared memory, all inter-CTA exchanges through distributed shared memory.
+// P column blocks resident in shared memory, small inter-CTA exchanges through distributed shared memory.
 #include <cooperative_groups.h>
 #include "hv_device_once.cuh"
 #include <math.h>
@@ -26,7 +26,7 @@ __global__ void __launch_bounds__(EK2_NT) ekf_check_batch_cluster2_kernel(EkfUpd
 {
     extern __shared__ __align__(16) double ek2_sm[];
     cg::cluster_group cluster = cg::this_cluster();
-    const int inst = blockIdx.x / (int)cluster.num_blocks();
+    const int inst = blockIdx.x / EK2_C;
     if (inst >= b.count) a = aug;                               // (one call of the body: its code is 340 KB)
     else {
         const EkfCheckItem& it = b.it[inst];
@@ -43,23 +43,18 @@ __global__ void __launch_bounds__(EK2_NT) ekf_check_batch_cluster2_kernel(EkfUpd
 #define EK2_STATIC_SMEM (sizeof(double) * (2 + EK2_LINV_DOUBLES + 2 + EK2_MAXN) + 256)
 #define EK2_SMEM_LIMIT (227 * 1024)
 
-// Cluster size 8 (the portable maximum). A 16-CTA cluster (non-portable size) halves the dense products but makes every
-// exchange slower.
-static int ek2_cluster_size() { return 8; }
-static int ek2_cluster_size_for(int, bool) { return 8; }
-
 bool ekf_cluster2_fits(int n, int l, int N, bool joseph)
 {
-    return N <= EK2_MAXN && ek2_smem_bytes(n, l, N, joseph, ek2_cluster_size()) + EK2_STATIC_SMEM <= EK2_SMEM_LIMIT;
+    return N <= EK2_MAXN && ek2_smem_bytes(n, l, N, joseph) + EK2_STATIC_SMEM <= EK2_SMEM_LIMIT;
 }
 
 template <class K, class... Args>
-static cudaError_t ek2_launch(K kernel, int C, int nclusters, size_t smem, cudaStream_t s, Args... args)
+static cudaError_t ek2_launch(K kernel, int nclusters, size_t smem, cudaStream_t s, Args... args)
 {
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(C * nclusters); cfg.blockDim = dim3(EK2_NT); cfg.dynamicSmemBytes = smem; cfg.stream = s;
+    cfg.gridDim = dim3(EK2_C * nclusters); cfg.blockDim = dim3(EK2_NT); cfg.dynamicSmemBytes = smem; cfg.stream = s;
     cudaLaunchAttribute at[2];
-    at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = C; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+    at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = EK2_C; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
     // programmatic dependent launch: this kernel may start while the previous KERNEL of the stream is still running (it waits
     // in griddepcontrol.wait before it reads the filter state); HV_EKF_NO_PDL=1 switches it off (A/B)
     static const bool pdl = getenv("HV_EKF_NO_PDL") == nullptr;
@@ -69,30 +64,25 @@ static cudaError_t ek2_launch(K kernel, int C, int nclusters, size_t smem, cudaS
 }
 
 template <class K>
-static cudaError_t ek2_prepare(K kernel, int C, size_t staticSmem = EK2_STATIC_SMEM)
+static cudaError_t ek2_prepare(K kernel)
 {
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(EK2_SMEM_LIMIT - staticSmem));
-    if (e != cudaSuccess) return e;
-    (void)C;
-    return cudaFuncSetAttribute(kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+    return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(EK2_SMEM_LIMIT - EK2_STATIC_SMEM));
 }
 
 cudaError_t ekf_launch_update_cluster2(const EkfUpdateArgs& a, cudaStream_t s)
 {
-    const int C = ek2_cluster_size_for(a.n, false);
     static bool seen[64];                             // per device (hv_common.cuh)
-    if (hv_first_use_on_device(seen)) { cudaError_t e = ek2_prepare(ekf_update_cluster2_kernel, C); if (e != cudaSuccess) return e; }
-    const size_t smem = ek2_smem_bytes(a.n, a.l, a.b.N, a.op == EKF_OP_AUGMENT, C);
-    return ek2_launch(ekf_update_cluster2_kernel, C, 1, smem, s, a);
+    if (hv_first_use_on_device(seen)) { cudaError_t e = ek2_prepare(ekf_update_cluster2_kernel); if (e != cudaSuccess) return e; }
+    const size_t smem = ek2_smem_bytes(a.n, a.l, a.b.N, a.op == EKF_OP_AUGMENT);
+    return ek2_launch(ekf_update_cluster2_kernel, 1, smem, s, a);
 }
 
 cudaError_t ekf_launch_check_batch2(const EkfUpdateArgs& a, const EkfCheckBatch& b, cudaStream_t s, const EkfUpdateArgs* aug)
 {
-    const int C = ek2_cluster_size();
     static bool seen[64];
-    if (hv_first_use_on_device(seen)) { cudaError_t e = ek2_prepare(ekf_check_batch_cluster2_kernel, C); if (e != cudaSuccess) return e; }
+    if (hv_first_use_on_device(seen)) { cudaError_t e = ek2_prepare(ekf_check_batch_cluster2_kernel); if (e != cudaSuccess) return e; }
     size_t smem = 0;
-    for (int i = 0; i < b.count; i++) { const size_t v = ek2_smem_bytes(b.it[i].n, b.it[i].l, a.b.N, false, C); if (v > smem) smem = v; }
-    if (aug) { const size_t v = ek2_smem_bytes(aug->n, aug->l, a.b.N, true, C); if (v > smem) smem = v; }
-    return ek2_launch(ekf_check_batch_cluster2_kernel, C, b.count + (aug ? 1 : 0), smem, s, a, b, aug ? *aug : a);
+    for (int i = 0; i < b.count; i++) { const size_t v = ek2_smem_bytes(b.it[i].n, b.it[i].l, a.b.N, false); if (v > smem) smem = v; }
+    if (aug) { const size_t v = ek2_smem_bytes(aug->n, aug->l, a.b.N, true); if (v > smem) smem = v; }
+    return ek2_launch(ekf_check_batch_cluster2_kernel, b.count + (aug ? 1 : 0), smem, s, a, b, aug ? *aug : a);
 }

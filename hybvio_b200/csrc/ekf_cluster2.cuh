@@ -1,17 +1,17 @@
-// hybvio_b200/csrc/ekf_cluster2.cuh -- body of the Kalman update / outlier check / pose augmentation kernel (cluster of C
+// hybvio_b200/csrc/ekf_cluster2.cuh -- body of the Kalman update / outlier check / pose augmentation kernel (cluster of 8
 // CTAs, fp64): second generation of ekf_cluster.cu. Same reference functions (src/odometry/ekf.cpp:57-82, 573-677,
 // 760-844, 848-885, 35-50) and the same algebra (elimination tableau [S | HP | v], Z = D^-1/2 L^-1 HP, P -= Z'Z, Joseph
 // form with the explicit 14-column T1); what changed is where the data lives and how the CTAs talk:
 //
 //   * CTA c owns the column block J_c of P and keeps ALL of it (N x B) in shared memory from the first load to the
 //     final store: P is read once and written once per update (the first generation re-read it for the downdate);
-//   * every exchange between CTAs goes through DISTRIBUTED SHARED MEMORY (cluster.map_shared_rank) instead of a
+//   * small exchanges between CTAs go through DISTRIBUTED SHARED MEMORY (cluster.map_shared_rank) instead of a
 //     write -> cluster barrier -> read round trip through L2:
-//       - innovation covariance: every CTA leaves its partial S in its own tableau; after one cluster barrier the
-//         partials are summed in a fixed order (bitwise identical in every CTA) -- directly by everybody when S is small
-//         (n*n <= 1024), otherwise reduce-scatter + all-gather;
-//       - the Z slices are gathered straight out of the neighbours' tableaus;
-//       - symmetrisation reads the mirrored entry from the owner's block; the Joseph form reads the 14 special columns
+//       - innovation covariance: when S is small (n*n <= 1024) every CTA leaves its partial S in shared memory and, after
+//         one cluster barrier, sums all of them itself in a fixed order (bitwise identical in every CTA); a larger S goes
+//         through L2 (partial slices -> reduced slices -> every CTA);
+//       - small Z slices are gathered straight out of the neighbours' tableaus (a large Z goes through L2);
+//       - symmetrisation sends every entry to the owner of its mirror image; the Joseph form reads the 14 special columns
 //         of G from the CTAs that own them;
 //   * the augmentation builds its shifted block A P A' + Q while loading (no P2 pass, no barrier), and a deferred
 //     maintainPositiveSemiDefinite() is applied in the same pass (EkfUpdateArgs::symFirst);
@@ -28,6 +28,7 @@
 #include "hv_dmma.cuh"
 
 #define EK2_NT 512
+#define EK2_C 8                       // CTAs per cluster (the portable maximum)
 #define EK2_MAXN 768
 #ifndef EK2_PHASE
 #define EK2_PHASE(i) do { } while (0)
@@ -37,17 +38,12 @@
 #define EK2_ELIM_DECL
 #endif
 
-struct Ek2Geom { int C, B, X, W, T, PB, RS, EXTRA, SYM, oneStage, LD; };
-#ifndef EK2_ODD_W                                     // (tools/: -DEK2_ODD_W measures the former layout)
+struct Ek2Geom { int B, X, W, T, PB, RS, EXTRA, SYM, oneStage, LD; };
 __host__ __device__ inline int ek2_pad4mod16(int w) { return w + ((20 - (w & 15)) & 15); }
-#else
-__host__ __device__ inline int ek2_pad4mod16(int w) { return w | 1; }
-#endif
-__host__ __device__ inline Ek2Geom ek2_geom(int n, int l, int N, bool joseph, int C)
+__host__ __device__ inline Ek2Geom ek2_geom(int n, int l, int N, bool joseph)
 {
     Ek2Geom g;
-    g.C = C;
-    g.B = (N + C - 1) / C;
+    g.B = (N + EK2_C - 1) / EK2_C;
     // Leading dimension of the P block and of the gathered Z: = 4 (mod 16) doubles, so that the DMMA fragment loads (8
     // consecutive + 4 strided elements per half-warp) touch 16 distinct 8-byte banks
     // (never N itself: column N of the gathered Z holds z_v for the CTA that updates the state mean)
@@ -61,17 +57,19 @@ __host__ __device__ inline Ek2Geom ek2_geom(int n, int l, int N, bool joseph, in
     g.T = (n * g.W + 1) & ~1;                               // even: the P block behind the tableau starts on a 16-byte boundary (bulk copies)
     g.PB = g.LD * g.B;                                      // own column block of P, ld LD
     const int MTn = (n + 7) >> 3;
-    const int E = (64 * (MTn * (MTn + 1) / 2) + C - 1) / C;    // two-stage: entries of the upper-triangular 8 x 8 tiles of S
-    // small S: every CTA leaves its partial in RS and sums all of them itself; else reduce-scatter (own slice in RS) + all-gather
+    const int E = (64 * (MTn * (MTn + 1) / 2) + EK2_C - 1) / EK2_C;   // two-stage: a slice of the upper-triangular 8 x 8 tiles of S
+    // small S: every CTA leaves its partial in RS and sums all of them itself; a large S goes through L2 and leaves RS unused
     g.oneStage = n * n <= 1024 ? 1 : 0;
-    g.RS = g.oneStage ? n * n : E;
+    g.RS = g.oneStage ? n * n : E;                          // (E unused; dropping it would move the cluster / single-CTA boundary, untimed)
     g.EXTRA = joseph ? N * EKF_POSE + 2 * 21 * g.LD + N * g.B : 0;   // K | [G special | K] | [T1c | R K] | P'' block
-    g.SYM = n <= 8 ? N * g.B : 0;                           // transposition buffer of the symmetrisation (its users have n <= 7)
+    // transposition buffer of the symmetrisation: present for every op that sets `symmetrize` (position 3 rows, zero height 1,
+    // orientation 4, augmentation 7), so the kernel needs no other way to reach the mirrored entries
+    g.SYM = n <= 8 ? N * g.B : 0;
     return g;
 }
-__host__ __device__ inline size_t ek2_smem_bytes(int n, int l, int N, bool joseph, int C)
+__host__ __device__ inline size_t ek2_smem_bytes(int n, int l, int N, bool joseph)
 {
-    const Ek2Geom g = ek2_geom(n, l, N, joseph, C);
+    const Ek2Geom g = ek2_geom(n, l, N, joseph);
     return ((size_t)g.X + g.T + g.PB + g.RS + g.EXTRA + g.SYM) * sizeof(double);
 }
 
@@ -388,18 +386,6 @@ __device__ __forceinline__ void ek2_pdl_wait()
 #endif
 }
 
-// Result words (VuOutlierStatus, chi2, numeric flag): device copy + optional mapped-host copy with a sequence flag
-__device__ __forceinline__ void ek2_report(const EkfUpdateArgs& a, double st, double chi2, double flag)
-{
-    a.b.res[0] = st; a.b.res[1] = chi2; a.b.res[2] = flag;
-    if (a.slot) { a.slot[0] = st; a.slot[1] = chi2; a.slot[2] = flag; }
-    if (a.sig) {
-        a.sig[0] = st; a.sig[1] = chi2; a.sig[2] = flag;
-        __threadfence_system();
-        ((volatile double*)a.sig)[3] = a.sigSeq;
-    }
-}
-
 // ---- bulk asynchronous copies (TMA, non-tensor form: cp.async.bulk) between global and shared memory, completion on an mbarrier.
 // One instruction moves a whole column / row / block: no register staging, no load -> store loop per thread. Addresses and sizes must
 // be multiples of 16 bytes (ek2_body checks and keeps the loops otherwise). On the host emulator: memcpy by the issuing thread.
@@ -481,15 +467,15 @@ __device__ __forceinline__ void ek2_body(EkfUpdateArgs& a, double* sm, Cluster c
     __shared__ int s_bad;
     __shared__ __align__(16) double s_m[EK2_MAXN];
     __shared__ __align__(8) unsigned long long s_bar[4];      // [0] staging (two arrivals: H, then P block + mean), [1] Z gather, [2] / [3] S exchange
-    const int c = (int)cluster.block_rank(), C = (int)cluster.num_blocks();
+    const int c = (int)cluster.block_rank(), C = (int)cluster.num_blocks();      // == EK2_C (as a run-time value: fewer spills)
     const int tid = threadIdx.x, lane = tid & 31, wrp = tid >> 5, nwarps = EK2_NT / 32;
     const int N = a.b.N, n = a.n, l = a.l;
     const bool joseph = a.op == EKF_OP_AUGMENT;
-    const Ek2Geom g = ek2_geom(n, l, N, joseph, C);
+    const Ek2Geom g = ek2_geom(n, l, N, joseph);
     double* X = sm;                 // H, later Z
     double* T = X + g.X;                                // tableau
     double* PB = T + g.T;                               // P[:, J_c]
-    double* RS = PB + g.PB;         // reduced S
+    double* RS = PB + g.PB;         // partial S (one-stage)
     double* EX = RS + g.RS;         // Joseph-form extras
     double* SYMB = EX + g.EXTRA;    // symmetrisation: mirrored entries, transposed
     const int W = g.W, B = g.B, LD = g.LD;
@@ -497,11 +483,12 @@ __device__ __forceinline__ void ek2_body(EkfUpdateArgs& a, double* sm, Cluster c
     const int vcol = n + B, cend = joseph ? vcol + n : vcol;
     const bool oneStage = g.oneStage != 0;
     // S exchange: entries of the upper-triangular 8 x 8 tiles, tile by tile (ETOT of them). Large S goes through L2 (bulk remote
-    // shared-memory pulls run at less than half the L2 rate): a.b.cwork = [ Z (N^2) | reduced S (N^2) | C partial S (8 N^2) ]
+    // shared-memory pulls run at less than half the L2 rate): a.b.cwork = [ Z (N^2) | reduced S (N^2) | C partial S (8 N^2) ].
+    // Precondition: the C partial slices of ETOT entries fit into 8 N^2, C ETOT <= 8 N^2, for every two-stage n <= N <= EK2_MAXN
+    // (tests/test_kalman_ref.py checks it).
     const int MTs = (n + 7) >> 3, ETOT = 64 * (MTs * (MTs + 1) / 2);
-    const bool bigS = !oneStage && a.b.cwork != nullptr && (size_t)C * ETOT <= (size_t)8 * N * N;
-    double* const Sred = a.b.cwork ? a.b.cwork + (size_t)N * N : nullptr;
-    double* const Spart = a.b.cwork ? a.b.cwork + (size_t)2 * N * N : nullptr;
+    double* const Sred = a.b.cwork + (size_t)N * N;
+    double* const Spart = a.b.cwork + (size_t)2 * N * N;
     double* const P = a.b.P;
 
     EK2_PHASE(0);
@@ -537,7 +524,7 @@ __device__ __forceinline__ void ek2_body(EkfUpdateArgs& a, double* sm, Cluster c
                 if (tid == 0) for (int q = arrived; q < 2; q++) ek2_bar_expect(&s_bar[0], 0);
                 ek2_bar_wait(&s_bar[0], 0);
             }
-            if (c == 0 && tid == 0) ek2_report(a, 1.0, 0.0, 0.0);
+            if (c == 0 && tid == 0) ekf_report(a, 1.0, 0.0, 0.0);
             return;
         }
     }
@@ -632,10 +619,10 @@ __device__ __forceinline__ void ek2_body(EkfUpdateArgs& a, double* sm, Cluster c
     if (checking && a.rmseThr >= 0.0) {               // ekf.cpp:797-801
         if (tid == 0) { double ss = 0.0; for (int i = 0; i < n; i++) { const double v = T[(size_t)i * W + vcol]; ss += v * v; } s_scalar[0] = sqrt(ss / n); }
         __syncthreads();
-        if (s_scalar[0] > a.rmseThr) { if (c == 0 && tid == 0) ek2_report(a, 2.0, 0.0, 0.0); return; }
+        if (s_scalar[0] > a.rmseThr) { if (c == 0 && tid == 0) ekf_report(a, 2.0, 0.0, 0.0); return; }
     }
     if (checking && a.skipChi2 && a.mode == EKF_MODE_CHECK) {
-        if (c == 0 && tid == 0) ek2_report(a, 0.0, 0.0, 0.0);
+        if (c == 0 && tid == 0) ekf_report(a, 0.0, 0.0, 0.0);
         return;
     }
 
@@ -654,15 +641,15 @@ __device__ __forceinline__ void ek2_body(EkfUpdateArgs& a, double* sm, Cluster c
                       [](int, int) { return 0.0; },
                       [&](int i, int j, double v0, double v1) {
                           if (oneStage) { RS[i * n + j] = v0; if (j + 1 < n) RS[i * n + j + 1] = v1; }      // partial stays out of the tableau
-                          else if (bigS) {                                                                  // tile-ordered, through L2
+                          else {                                                                            // tile-ordered, through L2
                               const int mt = i >> 3, nt = j >> 3;
                               double* dst = Spart + (size_t)c * ETOT + 64 * (nt * (nt + 1) / 2 + mt) + 8 * (i & 7) + (j & 7);
                               dst[0] = v0; dst[1] = v1;
-                          } else { T[(size_t)i * W + j] = v0; if (j + 1 < n) T[(size_t)i * W + j + 1] = v1; }
+                          }
                       });
     }
     EK2_PHASE(3);
-    if (bigS && bulk) ek2_fence_async_all();          // the partials are read by the neighbours' bulk copies
+    if (!oneStage && bulk) ek2_fence_async_all();     // the partials are read by the neighbours' bulk copies
     cluster.sync();                                   // #1: every partial S is in place (and from here on shared memory is exposed)
     // ---- reduce S through distributed shared memory, fixed order r = 0 .. C-1 (+ R on the diagonal)
     {
@@ -678,7 +665,7 @@ __device__ __forceinline__ void ek2_body(EkfUpdateArgs& a, double* sm, Cluster c
                 }
             }
             __syncthreads();
-        } else if (bigS && bulk && ETOT >= 2048 && ETOT % (2 * C) == 0 && 2 * ETOT <= g.X) {
+        } else if (bulk && ETOT >= 2048 && ETOT % (2 * C) == 0 && 2 * ETOT <= g.X) {
             // Through L2 with bulk copies: the eight partial slices and, after the second barrier, the reduced S arrive in the region H
             // occupied (dead since the partial product) by ONE round trip each, instead of one dependent load per entry and turn
             // (n = 84: 5.4 -> 4.4 us; below ~57 rows the barriers of the copies cost more than they save: n = 40 measured 2.8 -> 3.6 us)
@@ -721,20 +708,18 @@ __device__ __forceinline__ void ek2_body(EkfUpdateArgs& a, double* sm, Cluster c
                 int i, ip; entry(e, i, ip);
                 double s = 0.0;
                 if (i < n && ip < n) {
-                    if (bigS) { for (int r = 0; r < C; r++) s += Spart[(size_t)r * ETOT + e]; }
-                    else { for (int r = 0; r < C; r++) s += cluster.map_shared_rank(T, r)[(size_t)i * W + ip]; }
+                    for (int r = 0; r < C; r++) s += Spart[(size_t)r * ETOT + e];
                     if (i == ip) s += a.Rdiag;
                 }
-                if (bigS) Sred[e] = s; else RS[e - e0] = s;
+                Sred[e] = s;
             }
-            cluster.sync();                               // #2: all slices reduced; nobody reads the partials any more
+            cluster.sync();                               // #2: all slices reduced
             for (int tu = wrp; tu < ETOT / 64; tu += nwarps) {            // one tile per warp and turn: the tile index is decoded once
                 int mt, nt; ek2_upper_tile(tu, mt, nt);
 #pragma unroll
                 for (int h = 0; h < 2; h++) {
                     const int q = lane + 32 * h, e = 64 * tu + q, i = 8 * mt + (q >> 3), ip = 8 * nt + (q & 7);
-                    const int r = e / E;
-                    if (i < n && ip < n) T[(size_t)i * W + ip] = bigS ? Sred[e] : cluster.map_shared_rank(RS, r)[e - r * E];
+                    if (i < n && ip < n) T[(size_t)i * W + ip] = Sred[e];
                 }
             }
             __syncthreads();
@@ -754,7 +739,7 @@ __device__ __forceinline__ void ek2_body(EkfUpdateArgs& a, double* sm, Cluster c
         for (int i = tid; i < n; i += EK2_NT) T[(size_t)i * W + i] += a.Rdiag2 - a.Rdiag;
         const bool bad2 = !ek2_block_eliminate(Xc, W2, n, n + 1, wrp, lane, s_linv, &s_bad);
         if (bad2) {                                   // uniform over the cluster
-            if (c == 0 && tid == 0) ek2_report(a, 1.0, 0.0, 1.0);
+            if (c == 0 && tid == 0) ekf_report(a, 1.0, 0.0, 1.0);
             cluster.sync();
             return;
         }
@@ -769,7 +754,7 @@ __device__ __forceinline__ void ek2_body(EkfUpdateArgs& a, double* sm, Cluster c
         __syncthreads();
         const double chi2c = s_scalar[1];
         const bool outlier = chi2c > a.chi2Thr;
-        if (c == 0 && tid == 0) ek2_report(a, outlier ? 3.0 : 0.0, chi2c, 0.0);
+        if (c == 0 && tid == 0) ekf_report(a, outlier ? 3.0 : 0.0, chi2c, 0.0);
         if (outlier) { cluster.sync(); return; }
         decided = true;
         __syncthreads();                              // s_scalar / s_linv are reused below
@@ -777,7 +762,7 @@ __device__ __forceinline__ void ek2_body(EkfUpdateArgs& a, double* sm, Cluster c
     // ---- blocked forward elimination of [S | HP_Jc | v | (I)]: the right part becomes Z = L^-1 (.)
     const bool bad = !ek2_block_eliminate(T, W, n, cend + 1, wrp, lane, s_linv, &s_bad);
     if (bad) {                                        // uniform over the cluster
-        if (c == 0 && tid == 0) ek2_report(a, 1.0, 0.0, 1.0);
+        if (c == 0 && tid == 0) ekf_report(a, 1.0, 0.0, 1.0);
         if (a.specP) {
             // results go to the second buffers, but cannot be computed: leave the UNCHANGED state there, so that adopting them equals a
             // skipped update (what the in-place path does when this elimination fails)
@@ -802,14 +787,14 @@ __device__ __forceinline__ void ek2_body(EkfUpdateArgs& a, double* sm, Cluster c
         // INLIER under the check's R has been reported already; chi2 here belongs to the update's R and is not reported
     } else if (checking) {
         const bool outlier = !a.skipChi2 && chi2 > a.chi2Thr;
-        if (c == 0 && tid == 0) ek2_report(a, outlier ? 3.0 : 0.0, chi2, 0.0);
+        if (c == 0 && tid == 0) ekf_report(a, outlier ? 3.0 : 0.0, chi2, 0.0);
         if (outlier || a.mode == EKF_MODE_CHECK) { cluster.sync(); return; }
-    } else if (c == 0 && tid == 0) ek2_report(a, 0.0, chi2, 0.0);
+    } else if (c == 0 && tid == 0) ekf_report(a, 0.0, chi2, 0.0);
 
     EK2_PHASE(6);
     // ---- gather Z (n x N, row-major) out of the neighbours' tableaus, then P[:, J_c] -= Z' Z[:, J_c] in shared memory
     double* Z = X;                                    // H is dead
-    if ((size_t)n * N >= 4096 && a.b.cwork) {
+    if ((size_t)n * N >= 4096) {
         // large Z: through L2 (a CTA pulls an L2-resident block faster than a remote shared-memory one); every CTA publishes its slice, cluster barrier (release / acquire covers global memory), bulk read
         double* Zg = a.b.cwork;
         for (int t = tid; t < n * Bc; t += EK2_NT) { const int k = t / Bc, jj = t - k * Bc; Zg[(size_t)k * N + J0 + jj] = T[(size_t)k * W + n + jj]; }
@@ -926,37 +911,22 @@ __device__ __forceinline__ void ek2_body(EkfUpdateArgs& a, double* sm, Cluster c
     }
     double* const Pdst = a.specP ? a.specP : P;
     if (a.symmetrize) {
-        if (g.SYM) {
-            // the mirrored entry of P(i, j) is P(j, i), held by the CTA that owns column i: every CTA SENDS the entries of its block to the
-            // owners of their mirror images (row j of the own column i -> slot (i, j) of the owner of column j), remote stores that are
-            // complete at the cluster barrier; the first version fetched them after the barrier (a dependent round trip per element)
-            if (joseph) __syncthreads();              // the Joseph product above wrote the block
-            for (int idx = tid; idx < N * Bc; idx += EK2_NT) {
-                const int jrow = idx % N, icol = idx / N, r = jrow / B;
-                cluster.map_shared_rank(SYMB, r)[(J0 + icol) + (size_t)(jrow - r * B) * N] = Pblk[jrow + (size_t)icol * ldb];
-            }
+        // the mirrored entry of P(i, j) is P(j, i), held by the CTA that owns column i: every CTA SENDS the entries of its block to the
+        // owners of their mirror images (row j of the own column i -> slot (i, j) of the owner of column j, the buffer g.SYM), remote
+        // stores that are complete at the cluster barrier; the first version fetched them after the barrier (a dependent round trip per element)
+        if (joseph) __syncthreads();                  // the Joseph product above wrote the block
+        for (int idx = tid; idx < N * Bc; idx += EK2_NT) {
+            const int jrow = idx % N, icol = idx / N, r = jrow / B;
+            cluster.map_shared_rank(SYMB, r)[(J0 + icol) + (size_t)(jrow - r * B) * N] = Pblk[jrow + (size_t)icol * ldb];
         }
         cluster.sync();                               // #5: every final block is in shared memory, every mirror image has arrived
         EK2_PHASE(15);
-        if (g.SYM) {
-            for (int idx = tid; idx < N * Bc; idx += EK2_NT) {
-                const int i = idx % N, jj = idx / N, j = J0 + jj;
-                double v = Pblk[i + (size_t)jj * ldb];
-                const double w = SYMB[idx];
-                if (i != j) v = i > j ? 0.5 * (v + w) : 0.5 * (w + v);
-                Pdst[i + (size_t)j * N] = v;
-            }
-        } else {
-            for (int idx = tid; idx < N * Bc; idx += EK2_NT) {
-                const int i = idx % N, j = J0 + idx / N;
-                double v = Pblk[i + (size_t)(idx / N) * ldb];
-                if (i != j) {
-                    const int r = i / B;                  // owner of column i, which holds P(j, i)
-                    const double w = cluster.map_shared_rank(Pblk, r)[j + (size_t)(i - r * B) * ldb];
-                    v = i > j ? 0.5 * (v + w) : 0.5 * (w + v);      // same operand order as P(i>j) + P(j<i) on both sides
-                }
-                Pdst[i + (size_t)j * N] = v;
-            }
+        for (int idx = tid; idx < N * Bc; idx += EK2_NT) {
+            const int i = idx % N, jj = idx / N, j = J0 + jj;
+            double v = Pblk[i + (size_t)jj * ldb];
+            const double w = SYMB[idx];
+            if (i != j) v = i > j ? 0.5 * (v + w) : 0.5 * (w + v);
+            Pdst[i + (size_t)j * N] = v;
         }
     } else if (bulk) {
         // (the downdate wrote the block with ordinary stores: fenced towards the bulk-copy engine right after it, a CTA barrier since)

@@ -144,14 +144,14 @@ int main(int argc, char**)
         c.H = H + t * Hs; c.f = f + t * 2 * TM_MAXOBS; c.y = ip + t * TM_MAXOBS * 2;
         c.Rdiag = chiR * chiR * noiseScale; c.chi2Thr = orc_chi2inv95(n);
         c.gateI = status + 4 * t + 1; c.gateIExpect = 0; c.counter = counter; c.counterMax = maxSucc; c.slot = slots + 8 * t; c.lateH = 1;
-        const size_t smem = ek2_smem_bytes(n, l, N, false, 8);
+        const size_t smem = ek2_smem_bytes(n, l, N, false);
         if (fused) { c.mode = EKF_MODE_CHECK_UPDATE; c.Rdiag2 = visR * visR * noiseScale; c.bump = counter; }
-        int bad = EMU_LAUNCH_CLUSTER(arena, 8, EK2_NT, smem, emu_chain_update_body, &c);
+        int bad = EMU_LAUNCH_CLUSTER(arena, EK2_C, EK2_NT, smem, emu_chain_update_body, &c);
         if (!fused) {
             EkfUpdateArgs u = c;
             u.mode = EKF_MODE_UPDATE; u.Rdiag = visR * visR * noiseScale; u.chi2Thr = 0.0;
             u.gateI = nullptr; u.counter = nullptr; u.gateD = slots + 8 * t; u.gateDExpect = 0.0; u.bump = counter; u.slot = slots + 8 * t + 4;
-            bad += EMU_LAUNCH_CLUSTER(arena, 8, EK2_NT, smem, emu_chain_update_body, &u);
+            bad += EMU_LAUNCH_CLUSTER(arena, EK2_C, EK2_NT, smem, emu_chain_update_body, &u);
         } else {
             slots[8 * t + 4] = (slots[8 * t] == 0.0 && slots[8 * t + 2] == 0.0) ? 0.0 : 1.0;      // "updated" as the host derives it in fused mode
         }

@@ -32,37 +32,35 @@ static double rnd() { return rand() / (double)RAND_MAX - 0.5; }
 static double gauss() { double s = 0; for (int i = 0; i < 12; i++) s += rand() / (double)RAND_MAX; return s - 6.0; }
 
 // gate: 0 none; 1 device-side gates present and satisfied (+ lateH, slot, bump); 2 / 3 / 4: gated off by the int flag / the counter / the double flag
-struct Case { const char* name; int trail, C, op, n, l, mode; double yscale; int symFirst, drop; int gate = 0; double r2 = 0.0; int second = 0; };   // second: results into specP / specM, P and m untouched   // r2 > 0: the update uses its own noise level (two-R check+update)
+struct Case { const char* name; int trail, op, n, l, mode; double yscale; int symFirst, drop; int gate = 0; double r2 = 0.0; int second = 0; };   // second: results into specP / specM, P and m untouched   // r2 > 0: the update uses its own noise level (two-R check+update)
 
 int main(int argc, char** argv)
 {
     const Case cases[] = {
-        {"dense n=8 check+update", 20, 8, EKF_OP_DENSE, 8, 34, EKF_MODE_CHECK_UPDATE, 0.02, 0, 0},
-        {"dense n=20 check (outlier)", 20, 8, EKF_OP_DENSE, 20, 55, EKF_MODE_CHECK, 40.0, 0, 0},
-        {"dense n=40 update", 20, 8, EKF_OP_DENSE, 40, 90, EKF_MODE_UPDATE, 0.02, 0, 0},
-        {"dense n=84 check+update", 20, 8, EKF_OP_DENSE, 84, 160, EKF_MODE_CHECK_UPDATE, 0.02, 0, 0},
-        {"dense n=20 update N=62", 6, 8, EKF_OP_DENSE, 20, 55, EKF_MODE_UPDATE, 0.02, 0, 0},
-        {"dense n=40 check+update C=16", 20, 16, EKF_OP_DENSE, 40, 90, EKF_MODE_CHECK_UPDATE, 0.02, 0, 0},
-        {"augment drop last + deferred symmetrise", 20, 8, EKF_OP_AUGMENT, 7, 27, EKF_MODE_UPDATE, 0, 1, -1},
-        {"augment drop 3 N=62", 6, 8, EKF_OP_AUGMENT, 7, 27, EKF_MODE_UPDATE, 0, 0, 3},
-        {"augment C=16", 20, 16, EKF_OP_AUGMENT, 7, 27, EKF_MODE_UPDATE, 0, 0, -1},
-        {"position update (symmetrise)", 20, 8, EKF_OP_POSITION, 3, 3, EKF_MODE_UPDATE, 0, 0, 0},
-        {"zupt", 6, 8, EKF_OP_ZUPT, 3, 6, EKF_MODE_UPDATE, 0, 0, 0},
-        {"dense n=120 update (batch visual update)", 30, 8, EKF_OP_DENSE, 120, 160, EKF_MODE_UPDATE, 0.02, 0, 0},
-        {"dense n=13 check+update N=62 (odd sizes)", 6, 8, EKF_OP_DENSE, 13, 41, EKF_MODE_CHECK_UPDATE, 0.02, 0, 0},
-        {"gated chain link: gates open, late H, update", 20, 8, EKF_OP_DENSE, 24, 97, EKF_MODE_UPDATE, 0.02, 0, 0, 1},
-        {"gated chain link: gates open, check", 20, 8, EKF_OP_DENSE, 24, 97, EKF_MODE_CHECK, 0.02, 0, 0, 1},
-        {"gated off by the model flag", 20, 8, EKF_OP_DENSE, 24, 97, EKF_MODE_CHECK, 0.02, 0, 0, 2},
-        {"gated off by the success counter", 20, 8, EKF_OP_DENSE, 24, 97, EKF_MODE_CHECK, 0.02, 0, 0, 3},
-        {"update gated off by the check result", 20, 8, EKF_OP_DENSE, 24, 97, EKF_MODE_UPDATE, 0.02, 0, 0, 4},
-        {"two-R check+update n=24 (inlier)", 20, 8, EKF_OP_DENSE, 24, 97, EKF_MODE_CHECK_UPDATE, 0.02, 0, 0, 0, 0.004},
-        {"two-R check+update n=24 (outlier)", 20, 8, EKF_OP_DENSE, 24, 97, EKF_MODE_CHECK_UPDATE, 40.0, 0, 0, 0, 0.004},
-        {"two-R check+update n=84 l=160", 20, 8, EKF_OP_DENSE, 84, 160, EKF_MODE_CHECK_UPDATE, 0.02, 0, 0, 0, 0.01},
-        {"two-R check+update n=8 (one-stage S), gated", 20, 8, EKF_OP_DENSE, 8, 34, EKF_MODE_CHECK_UPDATE, 0.02, 0, 0, 1, 0.2},
-        {"two-R check+update n=13 N=62", 6, 8, EKF_OP_DENSE, 13, 41, EKF_MODE_CHECK_UPDATE, 0.02, 0, 0, 0, 0.004},
-        {"augment + deferred symmetrise into the second buffers", 20, 8, EKF_OP_AUGMENT, 7, 27, EKF_MODE_UPDATE, 0, 1, -1, 0, 0.0, 1},
-        {"augment drop 2 N=62 into the second buffers", 6, 8, EKF_OP_AUGMENT, 7, 27, EKF_MODE_UPDATE, 0, 0, 2, 0, 0.0, 1},
-        {"two-R check+update n=40 into the second buffers", 20, 8, EKF_OP_DENSE, 40, 90, EKF_MODE_CHECK_UPDATE, 0.02, 0, 0, 0, 0.004, 1},
+        {"dense n=8 check+update", 20, EKF_OP_DENSE, 8, 34, EKF_MODE_CHECK_UPDATE, 0.02, 0, 0},
+        {"dense n=20 check (outlier)", 20, EKF_OP_DENSE, 20, 55, EKF_MODE_CHECK, 40.0, 0, 0},
+        {"dense n=40 update", 20, EKF_OP_DENSE, 40, 90, EKF_MODE_UPDATE, 0.02, 0, 0},
+        {"dense n=84 check+update", 20, EKF_OP_DENSE, 84, 160, EKF_MODE_CHECK_UPDATE, 0.02, 0, 0},
+        {"dense n=20 update N=62", 6, EKF_OP_DENSE, 20, 55, EKF_MODE_UPDATE, 0.02, 0, 0},
+        {"augment drop last + deferred symmetrise", 20, EKF_OP_AUGMENT, 7, 27, EKF_MODE_UPDATE, 0, 1, -1},
+        {"augment drop 3 N=62", 6, EKF_OP_AUGMENT, 7, 27, EKF_MODE_UPDATE, 0, 0, 3},
+        {"position update (symmetrise)", 20, EKF_OP_POSITION, 3, 3, EKF_MODE_UPDATE, 0, 0, 0},
+        {"zupt", 6, EKF_OP_ZUPT, 3, 6, EKF_MODE_UPDATE, 0, 0, 0},
+        {"dense n=120 update (batch visual update)", 30, EKF_OP_DENSE, 120, 160, EKF_MODE_UPDATE, 0.02, 0, 0},
+        {"dense n=13 check+update N=62 (odd sizes)", 6, EKF_OP_DENSE, 13, 41, EKF_MODE_CHECK_UPDATE, 0.02, 0, 0},
+        {"gated chain link: gates open, late H, update", 20, EKF_OP_DENSE, 24, 97, EKF_MODE_UPDATE, 0.02, 0, 0, 1},
+        {"gated chain link: gates open, check", 20, EKF_OP_DENSE, 24, 97, EKF_MODE_CHECK, 0.02, 0, 0, 1},
+        {"gated off by the model flag", 20, EKF_OP_DENSE, 24, 97, EKF_MODE_CHECK, 0.02, 0, 0, 2},
+        {"gated off by the success counter", 20, EKF_OP_DENSE, 24, 97, EKF_MODE_CHECK, 0.02, 0, 0, 3},
+        {"update gated off by the check result", 20, EKF_OP_DENSE, 24, 97, EKF_MODE_UPDATE, 0.02, 0, 0, 4},
+        {"two-R check+update n=24 (inlier)", 20, EKF_OP_DENSE, 24, 97, EKF_MODE_CHECK_UPDATE, 0.02, 0, 0, 0, 0.004},
+        {"two-R check+update n=24 (outlier)", 20, EKF_OP_DENSE, 24, 97, EKF_MODE_CHECK_UPDATE, 40.0, 0, 0, 0, 0.004},
+        {"two-R check+update n=84 l=160", 20, EKF_OP_DENSE, 84, 160, EKF_MODE_CHECK_UPDATE, 0.02, 0, 0, 0, 0.01},
+        {"two-R check+update n=8 (one-stage S), gated", 20, EKF_OP_DENSE, 8, 34, EKF_MODE_CHECK_UPDATE, 0.02, 0, 0, 1, 0.2},
+        {"two-R check+update n=13 N=62", 6, EKF_OP_DENSE, 13, 41, EKF_MODE_CHECK_UPDATE, 0.02, 0, 0, 0, 0.004},
+        {"augment + deferred symmetrise into the second buffers", 20, EKF_OP_AUGMENT, 7, 27, EKF_MODE_UPDATE, 0, 1, -1, 0, 0.0, 1},
+        {"augment drop 2 N=62 into the second buffers", 6, EKF_OP_AUGMENT, 7, 27, EKF_MODE_UPDATE, 0, 0, 2, 0, 0.0, 1},
+        {"two-R check+update n=40 into the second buffers", 20, EKF_OP_DENSE, 40, 90, EKF_MODE_CHECK_UPDATE, 0.02, 0, 0, 0, 0.004, 1},
     };
     const int only = argc > 1 ? atoi(argv[1]) : -1;
     int fails = 0, idx = -1;
@@ -136,7 +134,7 @@ int main(int argc, char** argv)
             a.Rdiag = 1e-2 * noiseScale;
             orc_ekf_update_zupt(o, 1e-2);
         }
-        const size_t smem = ek2_smem_bytes(cs.n, cs.l, N, cs.op == EKF_OP_AUGMENT, cs.C);
+        const size_t smem = ek2_smem_bytes(cs.n, cs.l, N, cs.op == EKF_OP_AUGMENT);
         double* P2 = nullptr; double* m2 = nullptr;
         std::vector<double> P0, m0;
         if (cs.second) {
@@ -146,7 +144,7 @@ int main(int argc, char** argv)
             a.specP = P2; a.specM = m2;
             P0.assign(P, P + (size_t)N * N); m0.assign(m, m + N);
         }
-        int bad = EMU_LAUNCH_CLUSTER(arena, cs.C, EK2_NT, smem, emu_update_body, &a);
+        int bad = EMU_LAUNCH_CLUSTER(arena, EK2_C, EK2_NT, smem, emu_update_body, &a);
         if (cs.second) {                                                   // the first buffers must be untouched; compare the second ones
             if (memcmp(P0.data(), P, sizeof(double) * (size_t)N * N) != 0 || memcmp(m0.data(), m, sizeof(double) * N) != 0) bad |= 64;
             P = P2; m = m2;
@@ -164,7 +162,7 @@ int main(int argc, char** argv)
             const int expectCounter = (cs.gate == 3 ? 5 : 2) + ((cs.gate == 1 && (cs.mode == EKF_MODE_UPDATE || (cs.mode == EKF_MODE_CHECK_UPDATE && ost == 0))) ? 1 : 0);
             ok = ok && gflag[1] == expectCounter;                                                          // bumped only by an applied update
         }
-        printf("[%2d] %-42s N=%3d C=%2d smem %6.1f KB: status %d/%d chi2 %.6g/%.6g  max|dm| %.2e  max|dP|/max|P| %.2e  %s\n", idx, cs.name, N, cs.C, smem / 1024.0,
+        printf("[%2d] %-42s N=%3d smem %6.1f KB: status %d/%d chi2 %.6g/%.6g  max|dm| %.2e  max|dP|/max|P| %.2e  %s\n", idx, cs.name, N, smem / 1024.0,
                (int)res[0], ost, res[1], ochi2, em, eP / pmax, ok ? "ok" : "FAIL");
         fflush(stdout);
         fails += !ok;

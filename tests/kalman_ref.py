@@ -178,7 +178,7 @@ def kappa_S(P, H, r, noise_scale):
 
 # ---------------------------------------------------------------------------------------------------------- kernel paths
 # Restatement of the launchers' predicates (hybvio_b200/csrc/ekf_cluster2.cu ekf_cluster2_fits, ekf_cluster2.cuh ek2_geom / ek2_body,
-# ekf.cu ekf_update_smem_bytes, ekf_capi.cu prep_update) for a dense visual measurement (no Joseph form).
+# ekf.cu ekf_update_smem_bytes / ekf_launch_update) for a dense visual measurement (no Joseph form).
 EK2_C, EK2_MAXN = 8, 768
 EK2_STATIC_SMEM = 8 * (2 + 128 + 2 + EK2_MAXN) + 256
 EK2_SMEM_LIMIT = 227 * 1024
@@ -189,7 +189,8 @@ def _pad4mod16(w):
     return w + ((20 - (w & 15)) & 15)
 
 
-def ek2_smem_bytes(n, l, N, C=EK2_C):
+def ek2_smem_bytes(n, l, N):
+    C = EK2_C
     B = (N + C - 1) // C
     LDp = N + (((20 - (N & 15)) & 15) or 16)
     X = n * max(l, LDp)
@@ -223,9 +224,7 @@ def kernel_path(n, l, N, h_aligned=True):
         MT = (n + 7) >> 3
         ETOT = 64 * (MT * (MT + 1) // 2)
         X = ek2_smem_bytes(n, l, N)[1]
-        if EK2_C * ETOT > 8 * N * N:
-            s = "two-stage-dsmem"                               # reduce-scatter through distributed shared memory
-        elif bulk and ETOT >= 2048 and ETOT % (2 * EK2_C) == 0 and 2 * ETOT <= X:
+        if bulk and ETOT >= 2048 and ETOT % (2 * EK2_C) == 0 and 2 * ETOT <= X:
             s = "two-stage-l2-bulk"
         else:
             s = "two-stage-l2"

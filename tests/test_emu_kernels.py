@@ -20,7 +20,7 @@ def test_predict_kernel_body_on_host_emulator(tmp_path):
 
 
 def test_cluster_update_kernel_body_on_host_emulator(tmp_path):
-    """ekf_cluster2.cuh (8 / 16 CTAs as forked processes, distributed shared memory as a shared mapping): dense check /
+    """ekf_cluster2.cuh (8 CTAs as forked processes, distributed shared memory as a shared mapping): dense check /
     update / check+update at n = 8..84, augmentation incl. the deferred symmetrisation, selector updates, and the device-side
     gates of a chain issued without host round trips (open; closed by the model flag / the success counter / the check result),
     check + update with two noise levels in one kernel, results into the second buffers (speculative update; augmentation
@@ -33,7 +33,7 @@ def test_cluster_update_kernel_body_on_host_emulator(tmp_path):
                            os.path.join(ROOT, "tests", "emu", "emu_update.cpp"), obj, "-lm", "-o", exe])
     out = subprocess.run([exe], capture_output=True, text=True, timeout=900)
     assert out.returncode == 0, out.stdout + out.stderr
-    assert out.stdout.count(" ok") == 26 and "FAIL" not in out.stdout
+    assert out.stdout.count(" ok") == 24 and "FAIL" not in out.stdout
 
 
 def test_track_model_kernel_body_on_host_emulator(tmp_path):
@@ -160,7 +160,7 @@ def test_kernel_bodies_are_race_free_under_thread_sanitizer(tmp_path):
     # (harness, oracle objects, argument lists, extra environment, cluster kernel?)
     runs = [("emu_track_model", ["hv_oracle_tri"], [[]], {}, False), ("emu_track_model", ["hv_oracle_tri"], [[]], {"EMU_NT": "512"}, False),
             ("emu_predict", ["hv_oracle_ekf"], [[]], {}, False), ("emu_lk", ["hv_oracle_lk"], [[]], {}, False), ("emu_pyramid", ["hv_oracle_lk"], [[]], {}, False),
-            ("emu_update", ["hv_oracle_ekf"], [["0"], ["3"], ["5"], ["6"], ["14"], ["20"], ["23"]], {}, True),
+            ("emu_update", ["hv_oracle_ekf"], [["0"], ["3"], ["5"], ["12"], ["18"], ["21"]], {}, True),
             ("emu_chain", ["hv_oracle_ekf", "hv_oracle_tri"], [[], ["fused"]], {}, True)]
     built = {}
     for src, deps, arglists, extra, cluster in runs:

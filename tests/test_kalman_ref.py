@@ -125,8 +125,8 @@ def test_path_predicates_match_the_documented_boundaries():
 
 def test_sweep_covers_every_reachable_kernel_path():
     """Every (kernel) x (S reduction) x (Z exchange) x (H / P staging) combination some dense visual shape reaches on the sweep's state
-    layouts is in the sweep, and so are both sides of each boundary. The reduce-scatter of S through distributed shared memory is not
-    reachable at any state dimension the filter supports."""
+    layouts is in the sweep, and so are both sides of each boundary. The last loop guards a precondition of the two-stage S reduction
+    through L2: the cluster's partial slices of S fit into the 8 N^2 doubles of the exchange buffer for every supported N."""
     shapes = K.sweep_shapes()
     got = {(K.state_dim(t, ms), K.kernel_path(n, l, K.state_dim(t, ms))) for t, ms, n, l in shapes}
     for t, ms in K.CONFIGS:

@@ -12,7 +12,7 @@ __global__ void __launch_bounds__(EK2_NT) k_gemm(double* gS, long long* out, int
     extern __shared__ __align__(16) double sm[];
     const int tid = threadIdx.x, lane = tid & 31, wrp = tid >> 5;
     const int n = 84, l = 160, N = 160, Bc = 20, J0 = 0;
-    const Ek2Geom g = ek2_geom(n, l, N, false, 8);
+    const Ek2Geom g = ek2_geom(n, l, N, false);
     double* X = sm; double* T = X + g.X; double* PB = T + g.T;
     const int W = g.W, LD = g.LD;
     for (int i = tid; i < g.X; i += EK2_NT) X[i] = 1e-3 * (i % 17);
@@ -46,7 +46,7 @@ int main()
     double* gS; long long* out;
     cudaMalloc(&gS, 8 * 8192); cudaMalloc(&out, 8 * 16);
     cudaFuncSetAttribute(k_gemm, cudaFuncAttributeMaxDynamicSharedMemorySize, 218 * 1024);
-    const size_t smem = ek2_smem_bytes(84, 160, 160, false, 8);
+    const size_t smem = ek2_smem_bytes(84, 160, 160, false);
     const char* names[4] = {"HP 84 x 20 x 160 (1320 DMMA: 5280 cycles at the tensor rate)", "partial S 84 x 84 x 20, upper tiles -> global (330 DMMA: 1320 cycles)",
                             "partial S -> shared memory", "downdate 160 x 21 x 84 (1260 DMMA: 5040 cycles)"};
     for (int v = 0; v < 4; v++) {

@@ -49,9 +49,8 @@ int main()
         a.b.m = dm; a.b.P = dP; a.b.res = dres; a.b.cwork = dcw; a.b.N = N; a.b.trail = trail;
         a.op = EKF_OP_DENSE; a.n = n; a.l = l; a.mode = EKF_MODE_UPDATE; a.noiseScale = 1e4; a.rmseThr = -1.0; a.H = dH; a.f = df; a.y = dy;
         a.Rdiag = 0.05 * 0.05 * 1e4; a.normalizeAll = 1;
-        const size_t smem = ek2_smem_bytes(n, l, N, false, 8);
+        const size_t smem = ek2_smem_bytes(n, l, N, false);
         { cudaError_t e0 = cudaFuncSetAttribute(k_rep, cudaFuncAttributeMaxDynamicSharedMemorySize, 212 * 1024); if (e0 != cudaSuccess) { printf("attr: %s\n", cudaGetErrorString(e0)); return 1; } }
-        cudaFuncSetAttribute(k_rep, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
         cudaLaunchConfig_t cfg = {};
         cfg.gridDim = dim3(8); cfg.blockDim = dim3(EK2_NT); cfg.dynamicSmemBytes = smem;
         cudaLaunchAttribute at[1];
