@@ -116,6 +116,8 @@ def load():
     lib.hv_gftt_cells.argtypes = [c_void_p, c_int, ctypes.POINTER(c_int), ctypes.POINTER(c_int)]
     lib.hv_gftt_detect.argtypes = [c_void_p, c_void_p, c_int, c_int, ctypes.c_float, c_void_p]
     lib.hv_gftt_detect_device.argtypes = [c_void_p, c_void_p, c_int, c_int, ctypes.c_float, c_void_p]
+    lib.hv_subpix_refine.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_double]
+    lib.hv_subpix_refine_device.argtypes = lib.hv_subpix_refine.argtypes
     _bind_ekf(lib)
     _lib = lib
     return lib
@@ -313,6 +315,21 @@ class Pyramid:
 
     def gftt_detect_device(self, d_kp, block_size=3, cell=32, min_response=1e-3):
         check(self.lib.hv_gftt_detect_device(self.ctx.h, self.h, block_size, cell, min_response, d_kp), "hv_gftt_detect_device")
+
+    def subpix_refine(self, xy, win=(5, 5), zero_zone=(-1, -1), criteria=(3, 30, 0.01)):
+        """cv::cornerSubPix on the level-0 image of this pyramid; criteria = (type: 1 COUNT | 2 EPS, max_count, epsilon).
+        Returns the refined points as a new (n, 2) float32 array."""
+        out = np.ascontiguousarray(xy, dtype=np.float32).reshape(-1, 2).copy()
+        check(self.lib.hv_subpix_refine(self.ctx.h, self.h, _ptr(out), len(out), win[0], win[1], zero_zone[0], zero_zone[1],
+                                        criteria[0], criteria[1], criteria[2]), "hv_subpix_refine")
+        return out
+
+    def subpix_refine_device(self, d_xy, win=(5, 5), zero_zone=(-1, -1), criteria=(3, 30, 0.01)):
+        """The same on a contiguous (n, 2) float32 CUDA tensor, refined in place on the context's stream (asynchronous)."""
+        assert d_xy.is_cuda and d_xy.is_contiguous() and d_xy.is_floating_point() and d_xy.element_size() == 4
+        n = d_xy.numel() // 2
+        check(self.lib.hv_subpix_refine_device(self.ctx.h, self.h, _ptr(d_xy), n, win[0], win[1], zero_zone[0], zero_zone[1],
+                                               criteria[0], criteria[1], criteria[2]), "hv_subpix_refine_device")
 
     def release(self):
         if self.h:

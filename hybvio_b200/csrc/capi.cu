@@ -1,6 +1,7 @@
 // hybvio_b200/csrc/capi.cu -- C ABI (include/hybvio_b200.h): context, image pyramid, Lucas-Kanade.
 // The EKF entry points live in ekf_capi.cu.
 #include "capi_internal.h"
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -489,6 +490,101 @@ int hv_gftt_detect(hv_ctx* c, hv_pyr* pyr, int blockSize, int cell, float minRes
         HV_CUDA(cudaStreamSynchronize(c->stream));
     }
     memcpy(kp, hs, bytes);
+    return HV_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ sub-pixel refinement (cornerSubPix)
+static int subpix_args(const char* who, hv_ctx* c, hv_pyr* pyr, int n, int hw, int hh, int zw, int zh, int criteriaType, int maxCount,
+                       double epsilon, SubpixArgs& a)
+{
+    if (!c || !pyr || pyr->ctx != c || n < 0) { hv_set_error("%s: invalid context / pyramid / count", who); return HV_ERR_INVALID; }
+    if (hw < 1 || hh < 1 || hw > HV_SUBPIX_MAX_HALF || hh > HV_SUBPIX_MAX_HALF) {
+        hv_set_error("%s: half-window %d x %d unsupported (1..%d per axis)", who, hw, hh, HV_SUBPIX_MAX_HALF);
+        return HV_ERR_UNSUPPORTED;
+    }
+    const HvLevel& L = pyr->desc.lv[0];
+    if (L.w < 2 * hw + 5 || L.h < 2 * hh + 5) {          // cv::cornerSubPix asserts it
+        hv_set_error("%s: image %d x %d smaller than the window needs (%d x %d)", who, L.w, L.h, 2 * hw + 5, 2 * hh + 5);
+        return HV_ERR_INVALID;
+    }
+    memset(&a, 0, sizeof(a));
+    a.gray = L.gray; a.pitch = L.gpitch; a.w = L.w; a.h = L.h; a.n = n; a.hw = hw; a.hh = hh;
+    // criteria and mask exactly as cv::cornerSubPix forms them (OpenCV's MIN / MAX macros; std::exp(float))
+    a.maxIters = 100;
+    if (criteriaType & 1) { a.maxIters = maxCount < 1 ? 1 : maxCount; a.maxIters = a.maxIters > 100 ? 100 : a.maxIters; }
+    double eps = (criteriaType & 2) ? (epsilon < 0. ? 0. : epsilon) : 0.;
+    a.eps2 = eps * eps;
+    const int ww = 2 * hw + 1, wh = 2 * hh + 1;
+    for (int i = 0; i < wh; i++) {
+        const float y = (float)(i - hh) / hh, vy = std::exp(-y * y);
+        for (int j = 0; j < ww; j++) {
+            const float x = (float)(j - hw) / hw;
+            a.mask[i * ww + j] = (float)(vy * std::exp(-x * x));
+        }
+    }
+    if (zw >= 0 && zh >= 0 && zw * 2 + 1 < ww && zh * 2 + 1 < wh)
+        for (int i = hh - zh; i <= hh + zh; i++)
+            for (int j = hw - zw; j <= hw + zw; j++) a.mask[i * ww + j] = 0.f;
+    return HV_OK;
+}
+
+int hv_subpix_refine_device(hv_ctx* c, hv_pyr* pyr, float* dXY, int n, int hw, int hh, int zw, int zh, int criteriaType, int maxCount,
+                            double epsilon)
+{
+    SubpixArgs a;
+    int rc = subpix_args("hv_subpix_refine_device", c, pyr, n, hw, hh, zw, zh, criteriaType, maxCount, epsilon, a);
+    if (rc != HV_OK) return rc;
+    if (n == 0) return HV_OK;
+    if (!dXY) { hv_set_error("hv_subpix_refine_device: NULL points"); return HV_ERR_INVALID; }
+    HV_CUDA(cudaSetDevice(c->device));
+    a.xy = (float2*)dXY;
+    HV_CUDA(hv_launch_subpix(a, c->stream));
+    c->launches += 1;
+    return HV_OK;
+}
+
+int hv_subpix_refine(hv_ctx* c, hv_pyr* pyr, float* xy, int n, int hw, int hh, int zw, int zh, int criteriaType, int maxCount, double epsilon)
+{
+    SubpixArgs a;
+    int rc = subpix_args("hv_subpix_refine", c, pyr, n, hw, hh, zw, zh, criteriaType, maxCount, epsilon, a);
+    if (rc != HV_OK) return rc;
+    if (n == 0) return HV_OK;
+    if (!xy) { hv_set_error("hv_subpix_refine: NULL points"); return HV_ERR_INVALID; }
+    for (int i = 0; i < n; i++) {
+        const float x = xy[2 * i], y = xy[2 * i + 1];
+        if (!(x >= 0.f && x < (float)a.w && y >= 0.f && y < (float)a.h)) {      // cv::cornerSubPix asserts it
+            hv_set_error("hv_subpix_refine: corner %d (%g, %g) outside the %d x %d image", i, x, y, a.w, a.h);
+            return HV_ERR_INVALID;
+        }
+    }
+    HV_CUDA(cudaSetDevice(c->device));
+    const size_t bytes = (size_t)n * 2 * sizeof(float);
+    rc = hv_ctx_reserve_stage(c, bytes);
+    if (rc != HV_OK) return rc;
+    uint8_t* hs = (uint8_t*)c->h_stage;
+    memcpy(hs, xy, bytes);
+    if (hv_polling_enabled()) {
+        // the kernel refines the points in the mapped pinned block itself and the last corner raises the flag (as the LK kernel does)
+        a.xy = (float2*)c->hd_stage;
+        volatile unsigned* flag = (volatile unsigned*)(hs + c->stageBytes);
+        a.doneCounter = c->d_done; c->doneCount += (unsigned)n; a.doneTarget = c->doneCount;
+        a.seq = ++c->seq; a.hostFlag = (volatile unsigned*)((uint8_t*)c->hd_stage + c->stageBytes);
+        HV_CUDA(hv_launch_subpix(a, c->stream));
+        c->launches += 1;
+        rc = hv_poll_flag(flag, a.seq, c->stream, "hv_subpix_refine");
+        if (rc != HV_OK) {
+            cudaStreamSynchronize(c->stream); cudaMemsetAsync(c->d_done, 0, sizeof(unsigned), c->stream); cudaStreamSynchronize(c->stream); c->doneCount = 0;
+            return rc;
+        }
+    } else {
+        a.xy = (float2*)c->d_stage;
+        HV_CUDA(cudaMemcpyAsync(c->d_stage, hs, bytes, cudaMemcpyHostToDevice, c->stream));
+        HV_CUDA(hv_launch_subpix(a, c->stream));
+        c->launches += 1;
+        HV_CUDA(cudaMemcpyAsync(hs, c->d_stage, bytes, cudaMemcpyDeviceToHost, c->stream));
+        HV_CUDA(cudaStreamSynchronize(c->stream));
+    }
+    memcpy(xy, hs, bytes);
     return HV_OK;
 }
 

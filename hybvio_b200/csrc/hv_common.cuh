@@ -85,6 +85,20 @@ struct GfttArgs {
 
 cudaError_t hv_launch_gftt(const GfttArgs& a, cudaStream_t stream);
 
+// ---- sub-pixel corner refinement launch description (subpix.cu)
+#define HV_SUBPIX_MAX_HALF 15        // half-window per axis: a 31 x 31 window at most
+struct SubpixArgs {
+    const uint8_t* gray; int pitch, w, h;
+    float2* xy; int n;                // refined in place; may be mapped pinned host memory
+    int hw, hh;                       // half-window (win.width, win.height)
+    int maxIters;                     // already clamped as cv::cornerSubPix does
+    double eps2;                      // already clamped and squared
+    float mask[(2 * HV_SUBPIX_MAX_HALF + 1) * (2 * HV_SUBPIX_MAX_HALF + 1)];    // (2 hh + 1) x (2 hw + 1), built on the host, zero zone applied
+    unsigned* doneCounter; unsigned doneTarget, seq; volatile unsigned* hostFlag;       // polled completion (like the LK kernel), optional
+};
+
+cudaError_t hv_launch_subpix(const SubpixArgs& a, cudaStream_t stream);
+
 // ---- frame ingest (ingest.cu)
 #define HV_REMAP_INVALID (-32768)
 struct HvRemapEntry { short x0, y0; float xfrac, yfrac; };      // 12 bytes per output pixel (hv_remap_entry of the C ABI)

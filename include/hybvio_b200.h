@@ -130,6 +130,21 @@ int hv_gftt_cells(const hv_pyr* pyr, int cell, int* cells_x, int* cells_y);
 int hv_gftt_detect(hv_ctx* ctx, hv_pyr* pyr, int block_size, int cell, float min_response, float* kp);
 int hv_gftt_detect_device(hv_ctx* ctx, hv_pyr* pyr, int block_size, int cell, float min_response, float* d_kp);
 
+/* ---------------------------------------------------------------- sub-pixel corner refinement --------------- */
+/* cv::cornerSubPix(level 0 of pyr, xy, Size(win_w, win_h), Size(zero_w, zero_h), TermCriteria(criteria_type, max_count, epsilon))
+ * (OCV/imgproc/src/cornersubpix.cpp): the SubPixelAdjuster step of the reference's detection (src/tracker/image.cpp:76-79) on the
+ * level-0 image that hv_pyr_build / hv_pyr_build_batch / hv_ingest_frame has already put into HBM. criteria_type: 1 COUNT, 2 EPS,
+ * 3 both (cv::TermCriteria values). Bit-identical to cv::cornerSubPix built without IPP.
+ *   xy        n x (x, y) float32, refined in place
+ * Errors: HV_ERR_UNSUPPORTED for a half-window outside 1..15 on either axis; HV_ERR_INVALID for NULL arguments, a pyramid of another
+ * context, or an image smaller than (2 win_w + 5) x (2 win_h + 5). hv_subpix_refine also returns HV_ERR_INVALID, before anything is
+ * launched, for a corner outside [0, w) x [0, h) (cv::cornerSubPix asserts); hv_subpix_refine_device cannot inspect its input and
+ * leaves such a corner unchanged. n = 0 launches nothing. */
+int hv_subpix_refine(hv_ctx* ctx, hv_pyr* pyr, float* xy, int n, int win_w, int win_h, int zero_w, int zero_h,
+                     int criteria_type, int max_count, double epsilon);          /* host xy in/out, synchronises */
+int hv_subpix_refine_device(hv_ctx* ctx, hv_pyr* pyr, float* d_xy, int n, int win_w, int win_h, int zero_w, int zero_h,
+                            int criteria_type, int max_count, double epsilon);   /* device xy, asynchronous */
+
 /* ---------------------------------------------------------------- frame ingest (SURVEY.md 8(f) N4) -------- */
 /* Device part of tracker::Image::Factory::build / buildStereo (src/tracker/image.cpp:243-308): colour -> gray
  * (accelerated-arrays pixelwiseAffine, image.cpp:360-366) and undistortion / rectification (UndistorterImplementation::undistort,
