@@ -116,6 +116,8 @@ def load():
     lib.hv_gftt_cells.argtypes = [c_void_p, c_int, ctypes.POINTER(c_int), ctypes.POINTER(c_int)]
     lib.hv_gftt_detect.argtypes = [c_void_p, c_void_p, c_int, c_int, ctypes.c_float, c_void_p]
     lib.hv_gftt_detect_device.argtypes = [c_void_p, c_void_p, c_int, c_int, ctypes.c_float, c_void_p]
+    lib.hv_gftt_select_device.argtypes = [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p]
+    lib.hv_gftt_corners.argtypes = [c_void_p, c_void_p, c_int, c_int, ctypes.c_float, c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p]
     lib.hv_subpix_refine.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_double]
     lib.hv_subpix_refine_device.argtypes = lib.hv_subpix_refine.argtypes
     _bind_ekf(lib)
@@ -254,6 +256,15 @@ class Context:
                                    1 if use_initial else 0, max_iter, eps, min_eig), "hv_lk_track")
         return out, status, ts
 
+    def gftt_select_device(self, d_kp, d_corners, d_count, d_prev=None, mask_radius=0, max_tracks=150):
+        """hv_gftt_select_device on contiguous CUDA tensors: d_kp (nkp, 3) float32 key points, d_prev (nprev, 2) float32 or None,
+        d_corners (capacity, 2) float32 and d_count (1,) int32 outputs; asynchronous on the context's stream."""
+        for t in (d_kp, d_corners, d_count) + (() if d_prev is None else (d_prev,)):
+            assert t.is_cuda and t.is_contiguous() and t.element_size() == 4
+        nprev = 0 if d_prev is None else d_prev.numel() // 2
+        check(self.lib.hv_gftt_select_device(self.h, _ptr(d_kp), d_kp.numel() // 3, _ptr(d_prev), nprev, mask_radius, max_tracks,
+                                             _ptr(d_corners), d_corners.numel() // 2, _ptr(d_count)), "hv_gftt_select_device")
+
     def lk_track_device(self, prev, nxt, d_prev, d_next, d_status, d_ts, n, use_initial, max_iter=20, eps=0.03, min_eig=1e-3):
         check(self.lib.hv_lk_track_device(self.h, prev.h, nxt.h, _ptr(d_prev), _ptr(d_next), _ptr(d_status), _ptr(d_ts), n,
                                           1 if use_initial else 0, max_iter, eps, min_eig), "hv_lk_track_device")
@@ -263,6 +274,11 @@ class Context:
         """The same launch on a stream of the caller; d_init (or None): predicted end points, read from their own buffer."""
         check(self.lib.hv_lk_track_device_on_stream(self.h, c_void_p(int(cuda_stream)), prev.h, nxt.h, _ptr(d_prev), _ptr(d_init), _ptr(d_next),
                                                     _ptr(d_status), _ptr(d_ts), n, max_iter, eps, min_eig), "hv_lk_track_device_on_stream")
+
+
+def gftt_select_capacity(nkp, mask_radius, max_tracks):
+    """Corner slots a selection over nkp key points can fill (the capacity hv_gftt_select_device / hv_gftt_corners require)."""
+    return min(max_tracks, 2 * nkp) if mask_radius > 0 else 2 * nkp
 
 
 def _stride0(im):
@@ -315,6 +331,17 @@ class Pyramid:
 
     def gftt_detect_device(self, d_kp, block_size=3, cell=32, min_response=1e-3):
         check(self.lib.hv_gftt_detect_device(self.ctx.h, self.h, block_size, cell, min_response, d_kp), "hv_gftt_detect_device")
+
+    def gftt_corners(self, prev=None, mask_radius=0, max_tracks=150, block_size=3, cell=32, min_response=1e-3):
+        """tracker::FeatureDetector::detect on the level-0 image of this pyramid: detection, stable sort, resize quirk and applyMinDistance
+        against `prev` ((nprev, 2) corners already tracked) on the device, one synchronisation. Returns the corners, (n, 2) float32."""
+        prev = np.zeros((0, 2), np.float32) if prev is None else np.ascontiguousarray(prev, np.float32).reshape(-1, 2)
+        cap = gftt_select_capacity(int(np.prod(self.gftt_cells(cell))), mask_radius, max_tracks)
+        out = np.zeros((max(cap, 1), 2), np.float32)
+        n = c_int(0)
+        check(self.lib.hv_gftt_corners(self.ctx.h, self.h, block_size, cell, min_response, _ptr(prev), len(prev), mask_radius, max_tracks,
+                                       _ptr(out), cap, ctypes.byref(n)), "hv_gftt_corners")
+        return out[:n.value].copy()
 
     def subpix_refine(self, xy, win=(5, 5), zero_zone=(-1, -1), criteria=(3, 30, 0.01)):
         """cv::cornerSubPix on the level-0 image of this pyramid; criteria = (type: 1 COUNT | 2 EPS, max_count, epsilon).

@@ -75,6 +75,7 @@ int hv_ctx_destroy(hv_ctx* c)
     if (c->d_stage) cudaFree(c->d_stage);
     if (c->h_stage) cudaFreeHost(c->h_stage);
     if (c->d_done) cudaFree(c->d_done);
+    if (c->d_selectScratch) cudaFree(c->d_selectScratch);
     if (c->d_ekfStage) cudaFree(c->d_ekfStage);
     if (c->h_ekfStage) cudaFreeHost(c->h_ekfStage);
     if (c->ownStream && c->stream) cudaStreamDestroy(c->stream);
@@ -490,6 +491,118 @@ int hv_gftt_detect(hv_ctx* c, hv_pyr* pyr, int blockSize, int cell, float minRes
         HV_CUDA(cudaStreamSynchronize(c->stream));
     }
     memcpy(kp, hs, bytes);
+    return HV_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ corner selection (N2)
+static_assert(HV_CORNER_NONE == HV_CORNER_NONE_F, "padding value of the header and of the kernel");
+
+// Checks the counts shared by both entry points (their pointers are checked by the callers first) and fills everything but the buffers;
+// *need = the slots the call can fill.
+static int select_args(const char* who, int nkp, int nprev, int maskRadius, int maxTracks, int capacity, GfttSelectArgs& a, int* need)
+{
+    if (nkp < 0 || nprev < 0 || maxTracks < 1) {
+        hv_set_error("%s: invalid count (nkp %d, nprev %d, max_tracks %d)", who, nkp, nprev, maxTracks);
+        return HV_ERR_INVALID;
+    }
+    if (nkp > HV_GFTT_SELECT_MAX_KP) { hv_set_error("%s: %d key points unsupported (at most %d)", who, nkp, HV_GFTT_SELECT_MAX_KP); return HV_ERR_UNSUPPORTED; }
+    if (maskRadius > HV_GFTT_SELECT_MAX_RADIUS) {
+        hv_set_error("%s: mask_radius %d unsupported (at most %d)", who, maskRadius, HV_GFTT_SELECT_MAX_RADIUS);
+        return HV_ERR_UNSUPPORTED;
+    }
+    const int all = 2 * nkp;
+    *need = maskRadius > 0 ? (maxTracks < all ? maxTracks : all) : all;
+    if (capacity < *need) { hv_set_error("%s: capacity %d below the %d corners the call can return", who, capacity, *need); return HV_ERR_INVALID; }
+    memset(&a, 0, sizeof(a));
+    a.nkp = nkp; a.nprev = nprev; a.maskRadius = maskRadius; a.maxTracks = maxTracks; a.capacity = capacity;
+    a.r2 = maskRadius > 0 ? (float)(maskRadius * maskRadius) : 0.f;             // applyMinDistance: float(maskRadius * maskRadius)
+    a.pow2 = 2;
+    while (a.pow2 < nkp) a.pow2 *= 2;
+    return HV_OK;
+}
+
+int hv_gftt_select_device(hv_ctx* c, const float* dKp, int nkp, const float* dPrev, int nprev, int maskRadius, int maxTracks, float* dCorners,
+                          int capacity, int* dCount)
+{
+    if (!c || !dCorners || !dCount || (nkp > 0 && !dKp) || (nprev > 0 && !dPrev)) {
+        hv_set_error("hv_gftt_select_device: NULL context or buffer");
+        return HV_ERR_INVALID;
+    }
+    GfttSelectArgs a;
+    int need = 0;
+    int rc = select_args("hv_gftt_select_device", nkp, nprev, maskRadius, maxTracks, capacity, a, &need);
+    if (rc != HV_OK) return rc;
+    HV_CUDA(cudaSetDevice(c->device));
+    a.kp = dKp; a.prev = dPrev; a.out = dCorners; a.count = dCount;
+    HV_CUDA(hv_launch_gftt_select(a, c->stream));      // nkp = 0: writes the count and the padding only
+    c->launches += 1;
+    return HV_OK;
+}
+
+int hv_gftt_corners(hv_ctx* c, hv_pyr* pyr, int blockSize, int cell, float minResponse, const float* prevXY, int nprev, int maskRadius,
+                    int maxTracks, float* corners, int capacity, int* count)
+{
+    GfttArgs g;
+    int rc = gftt_args("hv_gftt_corners", c, pyr, blockSize, cell, minResponse, g);
+    if (rc != HV_OK) return rc;
+    if (!corners || !count || (nprev > 0 && !prevXY)) { hv_set_error("hv_gftt_corners: NULL buffer"); return HV_ERR_INVALID; }
+    const int nkp = (g.w / cell) * (g.h / cell);
+    GfttSelectArgs a;
+    int need = 0;
+    rc = select_args("hv_gftt_corners", nkp, nprev, maskRadius, maxTracks, capacity, a, &need);
+    if (rc != HV_OK) return rc;
+    int got = 0;
+    if (nkp > 0) {
+        HV_CUDA(cudaSetDevice(c->device));
+        // device scratch: [key points 3 nkp | previous corners 2 nprev] floats; the key points never leave the device
+        const size_t scratch = sizeof(float) * (3 * (size_t)nkp + 2 * (size_t)nprev);
+        if (scratch > c->selectScratchBytes) {
+            if (c->d_selectScratch) { HV_CUDA(cudaStreamSynchronize(c->stream)); cudaFree(c->d_selectScratch); }
+            c->d_selectScratch = nullptr; c->selectScratchBytes = 0;
+            size_t cap = 4096; while (cap < scratch) cap *= 2;
+            HV_CUDA(cudaMalloc(&c->d_selectScratch, cap));
+            c->selectScratchBytes = cap;
+        }
+        // staging block: [previous corners 8 nprev | count (16 bytes) | corners 8 need]
+        const size_t oCount = (8 * (size_t)nprev + 15) / 16 * 16, oCorners = oCount + 16, total = oCorners + 8 * (size_t)need;
+        rc = hv_ctx_reserve_stage(c, total);
+        if (rc != HV_OK) return rc;
+        uint8_t* hs = (uint8_t*)c->h_stage; uint8_t* ds = (uint8_t*)c->d_stage;
+        float* dKp = c->d_selectScratch;
+        if (nprev > 0) {
+            memcpy(hs, prevXY, 8 * (size_t)nprev);
+            HV_CUDA(cudaMemcpyAsync(dKp + 3 * (size_t)nkp, hs, 8 * (size_t)nprev, cudaMemcpyHostToDevice, c->stream));
+        }
+        g.kp = dKp;
+        HV_CUDA(hv_launch_gftt(g, c->stream));
+        c->launches += 1;
+        a.kp = dKp; a.prev = dKp + 3 * (size_t)nkp; a.capacity = need;
+        if (hv_polling_enabled()) {
+            // the select kernel writes the corners and the count straight into the mapped pinned block and raises the flag
+            uint8_t* hd = (uint8_t*)c->hd_stage;
+            a.out = (float*)(hd + oCorners); a.count = (int*)(hd + oCount);
+            volatile unsigned* flag = (volatile unsigned*)(hs + c->stageBytes);
+            a.doneCounter = c->d_done; c->doneCount += 1u; a.doneTarget = c->doneCount;
+            a.seq = ++c->seq; a.hostFlag = (volatile unsigned*)(hd + c->stageBytes);
+            HV_CUDA(hv_launch_gftt_select(a, c->stream));
+            c->launches += 1;
+            rc = hv_poll_flag(flag, a.seq, c->stream, "hv_gftt_corners");
+            if (rc != HV_OK) {
+                cudaStreamSynchronize(c->stream); cudaMemsetAsync(c->d_done, 0, sizeof(unsigned), c->stream); cudaStreamSynchronize(c->stream); c->doneCount = 0;
+                return rc;
+            }
+        } else {
+            a.out = (float*)(ds + oCorners); a.count = (int*)(ds + oCount);
+            HV_CUDA(hv_launch_gftt_select(a, c->stream));
+            c->launches += 1;
+            HV_CUDA(cudaMemcpyAsync(hs + oCount, ds + oCount, total - oCount, cudaMemcpyDeviceToHost, c->stream));
+            HV_CUDA(cudaStreamSynchronize(c->stream));
+        }
+        memcpy(&got, hs + oCount, sizeof(int));
+        memcpy(corners, hs + oCorners, 8 * (size_t)got);
+    }
+    for (size_t i = 2 * (size_t)got; i < 2 * (size_t)capacity; i++) corners[i] = HV_CORNER_NONE;
+    *count = got;
     return HV_OK;
 }
 

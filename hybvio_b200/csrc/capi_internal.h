@@ -27,6 +27,7 @@ struct hv_ctx {
     // LK staging (host-buffer API): one pinned block + one device block, grown on demand
     void* h_stage = nullptr; void* d_stage = nullptr; size_t stageBytes = 0;
     void* hd_stage = nullptr;          // device alias of h_stage (mapped pinned memory): results are written straight to the host
+    float* d_selectScratch = nullptr; size_t selectScratchBytes = 0;     // hv_gftt_corners: key points and previous corners (device)
     unsigned* d_done = nullptr;        // completion counter of the polled launches (device)
     unsigned doneCount = 0, seq = 0;   // host mirror of the counter / sequence number of the last polled launch
     // EKF staging

@@ -85,6 +85,23 @@ struct GfttArgs {
 
 cudaError_t hv_launch_gftt(const GfttArgs& a, cudaStream_t stream);
 
+// ---- corner selection launch description (gftt_select.cu): the detector's sort, resize quirk and applyMinDistance
+#define HV_GFTT_SELECT_MAX_KP 16384   // key points per call: one CTA, the sort keys in opt-in shared memory (128 KB)
+#define HV_GFTT_SELECT_MAX_RADIUS 46340   // mask_radius^2 still fits the reference's int product
+#define HV_CORNER_NONE_F (-1.0e6f)    // padding slots [count, capacity) (HV_CORNER_NONE of the header)
+struct GfttSelectArgs {
+    const float* kp; int nkp;         // (x, y, response) per cell, as hv_launch_gftt writes them
+    const float* prev; int nprev;     // previous corners (x, y)
+    int maskRadius, maxTracks;
+    float r2;                         // (float)(mask_radius * mask_radius), formed on the host as the reference does
+    int pow2;                         // sort width: the smallest power of two >= nkp (>= 2)
+    float* out; int capacity;         // (x, y) per slot; may be mapped pinned host memory
+    int* count;                       // may be mapped pinned host memory
+    unsigned* doneCounter; unsigned doneTarget, seq; volatile unsigned* hostFlag;      // polled completion (like the LK kernel), optional
+};
+
+cudaError_t hv_launch_gftt_select(const GfttSelectArgs& a, cudaStream_t stream);
+
 // ---- sub-pixel corner refinement launch description (subpix.cu)
 #define HV_SUBPIX_MAX_HALF 15        // half-window per axis: a 31 x 31 window at most
 struct SubpixArgs {
