@@ -34,8 +34,45 @@ static double gauss() { double s = 0; for (int i = 0; i < 12; i++) s += rand() /
 // gate: 0 none; 1 device-side gates present and satisfied (+ lateH, slot, bump); 2 / 3 / 4: gated off by the int flag / the counter / the double flag
 struct Case { const char* name; int trail, op, n, l, mode; double yscale; int symFirst, drop; int gate = 0; double r2 = 0.0; int second = 0; };   // second: results into specP / specM, P and m untouched   // r2 > 0: the update uses its own noise level (two-R check+update)
 
+// File mode (tests/test_ekf_ops_ref.py): one fixed-H update or augmentation of a given state. The input holds 17 doubles (op code
+// 1..7 = zupt, zrupt, pseudo-velocity, position, zero height, orientation, augmentation; N, trail, mapDim, drop index, symFirst,
+// normalizeAll, symmetrize, Rdiag, noiseScale, augNoisePos, augNoiseOri, defaultSpeed, ysmall[4]), then m (N) and P (N x N,
+// column-major); the output holds m and P after the kernel body.
+static int run_file(const char* in, const char* out)
+{
+    FILE* fi = fopen(in, "rb");
+    if (!fi) { printf("cannot open %s\n", in); return 1; }
+    double h[17];
+    if (fread(h, sizeof(double), 17, fi) != 17) { fclose(fi); return 1; }
+    const int code = (int)h[0], N = (int)h[1];
+    static const int ops[8] = {-1, EKF_OP_ZUPT, EKF_OP_ZRUPT, EKF_OP_PSEUDO_VELOCITY, EKF_OP_POSITION, EKF_OP_ZERO_HEIGHT, EKF_OP_ORIENTATION, EKF_OP_AUGMENT};
+    static const int ns[8] = {0, 3, 3, 1, 3, 1, 4, 7}, ls[8] = {0, EKF_VEL + 3, EKF_BGA + 3, EKF_VEL + 2, EKF_POS + 3, EKF_POS + 3, EKF_ORI + 4, EKF_CAM + EKF_POSE};
+    if (code < 1 || code > 7 || N < EKF_CAM + EKF_POSE || N > EK2_MAXN) { fclose(fi); printf("bad header\n"); return 1; }
+    emu::Arena arena((size_t)64 << 20);
+    double* m = arena.alloc<double>(N); double* P = arena.alloc<double>((size_t)N * N);
+    double* res = arena.alloc<double>(64); double* cwork = arena.alloc<double>((size_t)10 * N * N);
+    const bool ok = fread(m, sizeof(double), N, fi) == (size_t)N && fread(P, sizeof(double), (size_t)N * N, fi) == (size_t)N * N;
+    fclose(fi);
+    if (!ok) return 1;
+    EkfUpdateArgs a; memset(&a, 0, sizeof(a));
+    a.b.m = m; a.b.P = P; a.b.res = res; a.b.cwork = cwork; a.b.N = N; a.b.trail = (int)h[2]; a.b.mapDim = (int)h[3];
+    a.op = ops[code]; a.n = ns[code]; a.l = ls[code]; a.mode = EKF_MODE_UPDATE; a.rmseThr = -1.0;
+    a.dropIdx = (int)h[4]; a.symFirst = (int)h[5]; a.normalizeAll = (int)h[6]; a.symmetrize = (int)h[7];
+    a.Rdiag = h[8]; a.noiseScale = h[9]; a.augNoisePos = h[10]; a.augNoiseOri = h[11]; a.defaultSpeed = h[12];
+    for (int i = 0; i < 4; i++) a.ysmall[i] = h[13 + i];
+    const int bad = EMU_LAUNCH_CLUSTER(arena, EK2_C, EK2_NT, ek2_smem_bytes(a.n, a.l, N, a.op == EKF_OP_AUGMENT), emu_update_body, &a);
+    FILE* fo = fopen(out, "wb");
+    if (!fo) return 1;
+    fwrite(m, sizeof(double), N, fo); fwrite(P, sizeof(double), (size_t)N * N, fo);
+    fclose(fo);
+    printf("file mode: op %d N=%d %s\n", code, N, bad == 0 ? "ok" : "FAIL");
+    munmap(arena.base, arena.size);
+    return bad;
+}
+
 int main(int argc, char** argv)
 {
+    if (argc == 4 && strcmp(argv[1], "file") == 0) return run_file(argv[2], argv[3]);
     const Case cases[] = {
         {"dense n=8 check+update", 20, EKF_OP_DENSE, 8, 34, EKF_MODE_CHECK_UPDATE, 0.02, 0, 0},
         {"dense n=20 check (outlier)", 20, EKF_OP_DENSE, 20, 55, EKF_MODE_CHECK, 40.0, 0, 0},

@@ -178,7 +178,8 @@ def kappa_S(P, H, r, noise_scale):
 
 # ---------------------------------------------------------------------------------------------------------- kernel paths
 # Restatement of the launchers' predicates (hybvio_b200/csrc/ekf_cluster2.cu ekf_cluster2_fits, ekf_cluster2.cuh ek2_geom / ek2_body,
-# ekf.cu ekf_update_smem_bytes / ekf_launch_update) for a dense visual measurement (no Joseph form).
+# ekf.cu ekf_update_smem_bytes / ekf_launch_update); joseph=True for the pose augmentation (the identity block in the tableau row and
+# the EXTRA buffers of the Joseph product).
 EK2_C, EK2_MAXN = 8, 768
 EK2_STATIC_SMEM = 8 * (2 + 128 + 2 + EK2_MAXN) + 256
 EK2_SMEM_LIMIT = 227 * 1024
@@ -189,23 +190,24 @@ def _pad4mod16(w):
     return w + ((20 - (w & 15)) & 15)
 
 
-def ek2_smem_bytes(n, l, N):
+def ek2_smem_bytes(n, l, N, joseph=False):
     C = EK2_C
     B = (N + C - 1) // C
     LDp = N + (((20 - (N & 15)) & 15) or 16)
     X = n * max(l, LDp)
-    W = _pad4mod16(n + B + 1)
+    W = _pad4mod16(n + B + 1 + (n if joseph else 0))
     T = (n * W + 1) & ~1
     PB = LDp * B
     MTn = (n + 7) >> 3
     E = (64 * (MTn * (MTn + 1) // 2) + C - 1) // C
     RS = n * n if n * n <= 1024 else E
+    EXTRA = N * 7 + 2 * 21 * LDp + N * B if joseph else 0
     SYM = N * B if n <= 8 else 0
-    return (X + T + PB + RS + SYM) * 8, X
+    return (X + T + PB + RS + EXTRA + SYM) * 8, X
 
 
-def cluster_fits(n, l, N):
-    return N <= EK2_MAXN and ek2_smem_bytes(n, l, N)[0] + EK2_STATIC_SMEM <= EK2_SMEM_LIMIT
+def cluster_fits(n, l, N, joseph=False):
+    return N <= EK2_MAXN and ek2_smem_bytes(n, l, N, joseph)[0] + EK2_STATIC_SMEM <= EK2_SMEM_LIMIT
 
 
 def kernel_path(n, l, N, h_aligned=True):

@@ -247,6 +247,47 @@ def test_kernel_identity_at_path_boundaries(hv, trail, ms, n):
     e.close()
 
 
+def _op_boundary_shapes():
+    """(trail, map points, op) on each side of the cluster / single-CTA boundary of the pose augmentation (Joseph form, N = 200 / 201)
+    and of the fixed-H updates (N = 323 / 324 for three and four rows, 328 / 329 for one row), from kalman_ref.cluster_fits."""
+    import ekf_ops_ref as E
+    out = []
+    for op, lo, hi in (("augment", (24, 4), (25, 2)), ("position", (42, 3), (43, 1)), ("orientation", (42, 3), (43, 1)),
+                       ("zero_height", (44, 0), (42, 5))):
+        assert E.update_kernel(op, K.state_dim(*lo)) == K.KERNEL_NAME["cluster"] and E.update_kernel(op, K.state_dim(*hi)) != K.KERNEL_NAME["cluster"]
+        out += [(*lo, op), (*hi, op)]
+    return out
+
+
+@pytest.mark.parametrize("trail,ms,op", _op_boundary_shapes())
+def test_kernel_identity_of_fixed_h_ops_at_path_boundaries(hv, trail, ms, op):
+    """The augmentation and the fixed-H updates launch the kernel the predicate (with the Joseph form's buffers for the augmentation)
+    names, on both sides of its boundary."""
+    import torch
+    from torch.profiler import profile, ProfilerActivity
+    from hybvio_b200 import capi
+    import ekf_ops_ref as E
+    N = K.state_dim(trail, ms)
+    m, P = K.make_state(trail, ms, 7, 27, KAPPA, 4)
+    call = {"augment": lambda e: e.augment(-1), "position": lambda e: e.update_position([0.1, -0.2, 0.05], 1e-3),
+            "orientation": lambda e: e.update_orientation([1.0, 0.0, 0.0, 0.0], 1e-2), "zero_height": lambda e: e.update_zero_height(1e-3)}[op]
+    e = capi.Ekf(hv, _params(trail, ms))
+    e.upload(m, P)
+    call(e)                                     # warm-up: function attributes, first launch
+    e.upload(m, P)
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        call(e)
+        e.download()
+        torch.cuda.synchronize()
+    e.close()
+    names = {ev.key.split("(")[0] for ev in prof.key_averages() if ev.key.startswith("ekf_")}
+    want = E.update_kernel(op, N)
+    other = {"ekf_update_cluster2_kernel", "ekf_update_kernel"} - {want}
+    print(f"\nKERNELS N={N} {op}: {sorted(names)} (predicate: {want})")
+    assert want in names and not (names & other), names
+
+
 @pytest.mark.parametrize("norm", [False, True])
 def test_predict_bursts_of_every_length(hv, oracle_lk, norm):
     """With set_imu_batching(16), bursts of k = 1..17 and 33 queued samples (one launch up to 16, then split), optionally with the
