@@ -539,7 +539,8 @@ cudaError_t ekf_launch_update(const EkfUpdateArgs& args, cudaStream_t s)
 {
     // 8-CTA cluster kernel (ekf_cluster2.cuh) whenever its shared-memory working set fits (n <= 84 at N = 160); the single-CTA
     // kernel below only for oversized measurements (batch updates with n up to N, tableau in global memory above 200 KB).
-    if (ekf_cluster2_fits(args.n, args.l, args.b.N, args.op == EKF_OP_AUGMENT)) return ekf_launch_update_cluster2(args, s);
+    // (rowChunk > 0: the row-chunked form of the cluster kernel, chosen by the caller for a measurement that does not fit it whole)
+    if (args.rowChunk > 0 || ekf_cluster2_fits(args.n, args.l, args.b.N, args.op == EKF_OP_AUGMENT)) return ekf_launch_update_cluster2(args, s);
     static bool seen[64];                             // per device: function attributes belong to the device's context
     if (hv_first_use_on_device(seen)) {
         cudaError_t e = cudaFuncSetAttribute(ekf_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);

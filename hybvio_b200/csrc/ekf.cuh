@@ -91,7 +91,10 @@ struct EkfUpdateArgs {
     const int* counter; int counterMax;
     int* bump;
     double* slot;
-    int lateH, padGate;
+    int lateH;
+    // Row-chunked form (ekf_cluster2.cuh, dense visual ops only; 0: off): the measurement is processed rowChunk rows at a time
+    // next to the resident P blocks, for measurements whose whole tableau does not fit shared memory (ek2_geom_chunked)
+    int rowChunk;
     // Results into the second buffers (ekf_cluster2.cuh; NULL: off): the updated covariance blocks and state mean are written to
     // specP / specM instead of P / m, which stay untouched -- the host adopts them by swapping pointers. Used by the speculative
     // update (dense check+update: adopted if the caller's updateVisualTrack(H, f, y, r) really follows the INLIER check with the same
@@ -164,8 +167,13 @@ struct EkfEwArgs {
 };
 
 cudaError_t ekf_launch_update(const EkfUpdateArgs& a, cudaStream_t s);
-// ekf_launch_update picks the cluster kernel (the only one with specP / specM, Rdiag2 and the device-side gates) iff this holds
+// ekf_launch_update picks the cluster kernel (the only one with specP / specM, Rdiag2 and the device-side gates) iff this holds or
+// a.rowChunk > 0
 bool ekf_cluster2_fits(int n, int l, int N, bool joseph);
+// Rows per pass of the row-chunked form of a dense visual op of shape (n, l): the largest height whose working set fits beside the
+// resident P blocks (n: one pass); 0 if not even min(n, EK2_MIN_CHUNK) rows fit
+int ekf_cluster2_chunk_rows(int n, int l, int N);
+// a.rowChunk > 0: the row-chunked form (whether or not the whole tableau would fit)
 cudaError_t ekf_launch_update_cluster2(const EkfUpdateArgs& a, cudaStream_t s);
 // aug != NULL: one more cluster of the same launch runs the augmentation *aug (results into aug->specP / aug->specM)
 cudaError_t ekf_launch_check_batch2(const EkfUpdateArgs& a, const EkfCheckBatch& b, cudaStream_t s, const EkfUpdateArgs* aug = nullptr);

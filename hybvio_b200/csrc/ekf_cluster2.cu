@@ -15,7 +15,14 @@ namespace cg = cooperative_groups;
 __global__ void __launch_bounds__(EK2_NT) ekf_update_cluster2_kernel(EkfUpdateArgs a)
 {
     extern __shared__ __align__(16) double ek2_sm[];
-    ek2_body(a, ek2_sm, cg::this_cluster());
+    ek2_body<false>(a, ek2_sm, cg::this_cluster());
+}
+
+// The row-chunked form (a.rowChunk > 0): a dense visual op whose whole tableau does not fit beside the P blocks
+__global__ void __launch_bounds__(EK2_NT) ekf_update_cluster2_chunked_kernel(EkfUpdateArgs a)
+{
+    extern __shared__ __align__(16) double ek2_sm[];
+    ek2_body<true>(a, ek2_sm, cg::this_cluster());
 }
 
 // Batched outlier checks: cluster i works on measurement i against the same state (read-only), with its own result words.
@@ -37,7 +44,7 @@ __global__ void __launch_bounds__(EK2_NT) ekf_check_batch_cluster2_kernel(EkfUpd
     }
     a.b.res += (size_t)EKF_RES_STRIDE * inst;
     a.b.cwork += (size_t)inst * 10 * a.b.N * a.b.N;           // own exchange area (Z | reduced S | partial S)
-    ek2_body(a, ek2_sm, cluster);
+    ek2_body<false>(a, ek2_sm, cluster);
 }
 
 #define EK2_STATIC_SMEM (sizeof(double) * (2 + EK2_LINV_DOUBLES + 2 + EK2_MAXN) + 256)
@@ -46,6 +53,14 @@ __global__ void __launch_bounds__(EK2_NT) ekf_check_batch_cluster2_kernel(EkfUpd
 bool ekf_cluster2_fits(int n, int l, int N, bool joseph)
 {
     return N <= EK2_MAXN && ek2_smem_bytes(n, l, N, joseph) + EK2_STATIC_SMEM <= EK2_SMEM_LIMIT;
+}
+
+int ekf_cluster2_chunk_rows(int n, int l, int N)
+{
+    if (N > EK2_MAXN) return 0;
+    for (int h = n; h >= 1 && h >= (n < EK2_MIN_CHUNK ? n : EK2_MIN_CHUNK); h--)      // (the working set grows with h)
+        if (ek2_smem_bytes_chunked(h, n, l, N) + EK2_STATIC_SMEM <= EK2_SMEM_LIMIT) return h;
+    return 0;
 }
 
 template <class K, class... Args>
@@ -71,7 +86,12 @@ static cudaError_t ek2_prepare(K kernel)
 
 cudaError_t ekf_launch_update_cluster2(const EkfUpdateArgs& a, cudaStream_t s)
 {
-    static bool seen[64];                             // per device (hv_common.cuh)
+    static bool seen[64], seenChunked[64];            // per device (hv_common.cuh)
+    if (a.rowChunk > 0) {
+        if (hv_first_use_on_device(seenChunked)) { cudaError_t e = ek2_prepare(ekf_update_cluster2_chunked_kernel); if (e != cudaSuccess) return e; }
+        const size_t smem = ek2_smem_bytes_chunked(a.rowChunk < a.n ? a.rowChunk : a.n, a.n, a.l, a.b.N);
+        return ek2_launch(ekf_update_cluster2_chunked_kernel, 1, smem, s, a);
+    }
     if (hv_first_use_on_device(seen)) { cudaError_t e = ek2_prepare(ekf_update_cluster2_kernel); if (e != cudaSuccess) return e; }
     const size_t smem = ek2_smem_bytes(a.n, a.l, a.b.N, a.op == EKF_OP_AUGMENT);
     return ek2_launch(ekf_update_cluster2_kernel, 1, smem, s, a);

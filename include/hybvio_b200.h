@@ -390,7 +390,11 @@ int hv_ekf_visual_track(hv_ekf* ekf, const hv_track_model* t, double r, double t
  * caller applies its own pre-filters (track score, trackMinFrames, blacklist, maxVisualUpdates: backend.cpp:1020-1047, 1241)
  * by choosing which tracks to submit. Results are those of the per-track calls hv_ekf_track_models ->
  * hv_ekf_visual_track(mode 0) -> hv_ekf_visual_track(mode 1) issued track by track.
- * Not covered: trackOutlierThresholdGrowthFactor != 1 (the thresholds are fixed for the chain), hybrid map points. */
+ * State sizes: a track whose measurement does not fit the cluster kernel whole (long trails, hybrid maps: at N = 202 tracks of more
+ * than 71 rows, N = 301 more than 41, N = 400 more than 16) runs in its row-chunked form, still one kernel for check and update.
+ * Every track of up to 84 rows (21 stereo poses) runs for N <= 424 (8-row tracks up to N = 432, 4-row up to 448); a chain with a track
+ * beyond that is refused with HV_ERR_UNSUPPORTED before anything is issued, the filter state untouched.
+ * Not covered: trackOutlierThresholdGrowthFactor != 1 (the thresholds are fixed for the chain), hybrid map-point tracks. */
 typedef struct hv_visual_update_params {
     double chi_outlier_r;            /* r of the check: odometry.trackChiTestOutlierR / focal length (backend.cpp:996) */
     double track_rmse_threshold;     /* odometry.trackRmseThreshold / focal length (backend.cpp:995); < 0: off */
