@@ -180,6 +180,7 @@ def _bind_ekf(lib):
     lib.hv_ekf_predicted_mean.argtypes = [c_void_p, c_void_p]
     lib.hv_ekf_run_device_results.argtypes = [c_void_p, c_int, ctypes.POINTER(c_int), ctypes.POINTER(c_double)]
     lib.hv_ekf_run_host.argtypes = [c_void_p, ctypes.POINTER(EkfOp), c_int, ctypes.POINTER(c_int), ctypes.POINTER(c_double), c_void_p]
+    lib.hv_ekf_group_run_device.argtypes = [ctypes.POINTER(c_void_p), c_int, ctypes.POINTER(ctypes.POINTER(EkfOp)), ctypes.POINTER(c_int)]
     lib.hv_ekf_normalize_quaternions.argtypes = [c_void_p, c_int]
     lib.hv_ekf_translate_to.argtypes = [c_void_p, c_void_p]
     lib.hv_ekf_transform_to.argtypes = [c_void_p, c_void_p, c_void_p, c_int]
@@ -200,6 +201,21 @@ def _ptr(a):
     if isinstance(a, np.ndarray):
         return a.ctypes.data
     return a.data_ptr()   # torch tensor
+
+
+GROUP_MAX = 64      # HV_EKF_GROUP_MAX
+
+
+def ekf_group_run_device(ekfs, lists):
+    """hv_ekf_group_run_device: steps several filters of one context with the launches of one. lists[i] is filter i's op list, as for
+    Ekf.run_device: an (EkfOp array, nops) pair or an EkfOp array (all of it). Asynchronous; raises HvError on a refusal (the filters
+    are then untouched and the caller steps them one by one)."""
+    n = len(ekfs)
+    pairs = [x if isinstance(x, tuple) else (x, len(x)) for x in lists]
+    E = (c_void_p * n)(*[e.h for e in ekfs])
+    O = (ctypes.POINTER(EkfOp) * n)(*[ctypes.cast(ops, ctypes.POINTER(EkfOp)) for ops, _ in pairs])
+    K = (c_int * n)(*[k for _, k in pairs])
+    check(load().hv_ekf_group_run_device(E, n, O, K), "hv_ekf_group_run_device")
 
 
 class Context:

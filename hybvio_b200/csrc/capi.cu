@@ -77,7 +77,10 @@ int hv_ctx_destroy(hv_ctx* c)
     if (c->d_done) cudaFree(c->d_done);
     if (c->d_selectScratch) cudaFree(c->d_selectScratch);
     if (c->d_ekfStage) cudaFree(c->d_ekfStage);
-    if (c->h_ekfStage) cudaFreeHost(c->h_ekfStage);
+    for (int i = 0; i < HV_EKF_STAGES; i++) {
+        if (c->h_ekfStage[i]) cudaFreeHost(c->h_ekfStage[i]);
+        if (c->evEkfStage[i]) cudaEventDestroy(c->evEkfStage[i]);
+    }
     if (c->ownStream && c->stream) cudaStreamDestroy(c->stream);
     delete c;
     return HV_OK;

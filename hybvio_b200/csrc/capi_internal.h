@@ -6,6 +6,7 @@
 #include <string>
 
 #define HV_TABLE_CAPACITY 1024   // pyramids per context
+#define HV_EKF_STAGES 4          // pinned staging blocks of hv_ekf_group_run_device per context (calls the host may run ahead)
 
 void hv_set_error(const char* fmt, ...);
 #define HV_CUDA(call)                                                                           \
@@ -30,8 +31,11 @@ struct hv_ctx {
     float* d_selectScratch = nullptr; size_t selectScratchBytes = 0;     // hv_gftt_corners: key points and previous corners (device)
     unsigned* d_done = nullptr;        // completion counter of the polled launches (device)
     unsigned doneCount = 0, seq = 0;   // host mirror of the counter / sequence number of the last polled launch
-    // EKF staging
-    void* h_ekfStage = nullptr; void* d_ekfStage = nullptr; size_t ekfStageBytes = 0;
+    // EKF group staging (hv_ekf_group_run_device): a call's argument blocks reach the device in one copy out of a ring of pinned blocks
+    // (block i is refilled once the copy out of it has completed, evEkfStage[i]) into one device block
+    void* h_ekfStage[HV_EKF_STAGES] = {}; size_t h_ekfStageBytes[HV_EKF_STAGES] = {}; cudaEvent_t evEkfStage[HV_EKF_STAGES] = {};
+    int ekfStageNext = 0;
+    void* d_ekfStage = nullptr; size_t ekfStageBytes = 0;
     // Side stream for work that the main stream need not wait for (created on first use; ekf_capi.cu: outlier checks of a device-resident
     // op list). hv_ctx_sync waits for both.
     cudaStream_t sideStream = nullptr;

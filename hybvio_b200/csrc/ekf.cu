@@ -356,6 +356,12 @@ __global__ void __launch_bounds__(EKF_NT) ekf_predict_kernel(EkfPredictArgs a)
     extern __shared__ __align__(16) double ekf_predict_dyn[];
     ekf_predict_body(a, ekf_predict_dyn);
 }
+// Group launch (hv_ekf_group_run_device): CTA i runs the IMU burst args[i] of one filter of the group (blocks in device memory)
+__global__ void __launch_bounds__(EKF_NT) ekf_group_predict_kernel(const EkfPredictArgs* __restrict__ args)
+{
+    extern __shared__ __align__(16) double ekf_predict_dyn[];
+    ekf_predict_body(args[blockIdx.x], ekf_predict_dyn);
+}
 
 // ------------------------------------------------------------------------------------------------ elementwise / structural
 __device__ __forceinline__ void quat_to_rot(const double* q /*w,x,y,z*/, double* R /*row-major*/)
@@ -573,6 +579,23 @@ cudaError_t ekf_launch_predict(const EkfPredictArgs& a, cudaStream_t s)
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = at; cfg.numAttrs = pdl ? 1 : 0;
     return cudaLaunchKernelEx(&cfg, ekf_predict_kernel, a);
+}
+cudaError_t ekf_launch_group_predict(const EkfPredictArgs* hArgs, const EkfPredictArgs* dArgs, int count, cudaStream_t s)
+{
+    static bool seen[64];
+    if (hv_first_use_on_device(seen)) {
+        cudaError_t e = cudaFuncSetAttribute(ekf_group_predict_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ekf_predict_smem_bytes(EKF_MAX_PREDICT));
+        if (e != cudaSuccess) return e;
+    }
+    int maxCount = 0;
+    for (int i = 0; i < count; i++) if (hArgs[i].count > maxCount) maxCount = hArgs[i].count;
+    static const bool pdl = getenv("HV_EKF_NO_PDL") == nullptr;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(count); cfg.blockDim = dim3(EKF_NT); cfg.dynamicSmemBytes = ekf_predict_smem_bytes(maxCount); cfg.stream = s;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = at; cfg.numAttrs = pdl ? 1 : 0;
+    return cudaLaunchKernelEx(&cfg, ekf_group_predict_kernel, dArgs);
 }
 cudaError_t ekf_launch_elementwise(const EkfEwArgs& a, cudaStream_t s)
 {

@@ -4,6 +4,7 @@
 #include "capi_internal.h"
 #include "ekf.cuh"
 #include "track_model.h"
+#include <algorithm>
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
@@ -144,11 +145,16 @@ extern "C" { static int staging_acquire(hv_ekf* e); }
 #define EKF_ENTER(e, who)                              \
     do { EKF_ENTER_LAZY(e, who); int rc2_ = flush_pending(e); if (rc2_ != HV_OK) return rc2_; } while (0)
 
-static int launch_update(hv_ekf* e, EkfUpdateArgs& a)
+// The filter's side of an update's argument block, at the moment it is issued
+static void update_settle(hv_ekf* e, EkfUpdateArgs& a)
 {
     e->epoch++;
     a.b = e->b;
     a.noiseScale = e->noiseScale;
+}
+static int launch_update(hv_ekf* e, EkfUpdateArgs& a)
+{
+    update_settle(e, a);
     HV_CUDA(ekf_launch_update(a, e->ctx->stream));
     e->ctx->launches++;
     return HV_OK;
@@ -462,11 +468,15 @@ static int join_cov(hv_ekf* e)
     e->covBusy = false;
     return HV_OK;
 }
+static void predict_settle(hv_ekf* e, EkfPredictArgs& a)
+{
+    a.b = e->b; a.gravity = e->prm.gravity;
+    e->epoch++;
+}
 static int predict_launch(hv_ekf* e, EkfPredictArgs& a)
 {
     if (a.count == 0) return HV_OK;
-    a.b = e->b; a.gravity = e->prm.gravity;
-    e->epoch++;
+    predict_settle(e, a);
     static const bool latencyMode = getenv("HV_EKF_NO_PDL") == nullptr;
     if (e->meanIssued && latencyMode) {
         // the mean of this burst is out already (hv_ekf_predicted_mean_device): the full launch runs beside the context's stream
@@ -780,11 +790,10 @@ int hv_ekf_visual_check_update(hv_ekf* e, const double* H, int n, int l, const d
     return visual_host(e, "hv_ekf_visual_check_update", H, n, l, f, y, r, rmseThr, EKF_MODE_CHECK_UPDATE, vuStatus, chi2, mOut);
 }
 
-static int visual_device(hv_ekf* e, const double* dH, int n, int l, const double* df, const double* dy, double r, double rmseThr,
-                         int mode, double* dResult, int lateH, double* slot = nullptr)
+static int visual_device_args(hv_ekf* e, const double* dH, int n, int l, const double* df, const double* dy, double r, double rmseThr,
+                              int mode, int lateH, double* slot, EkfUpdateArgs& a)
 {
     if (!dH || !df || !dy || mode < 0 || mode > 2) { hv_set_error("hv_ekf_visual_device: invalid argument"); return HV_ERR_INVALID; }
-    EkfUpdateArgs a;
     int rc = visual_args(e, "hv_ekf_visual_device", n, l, r, rmseThr, mode, a);
     if (rc != HV_OK) return rc;
     a.H = dH; a.f = df; a.y = dy;
@@ -792,6 +801,14 @@ static int visual_device(hv_ekf* e, const double* dH, int n, int l, const double
     // so it is staged AFTER griddepcontrol.wait; early staging is kept for H that arrived through the library's own H2D copy
     a.lateH = lateH;
     a.slot = slot;                                                 // the kernel writes its result words into the slot itself
+    return HV_OK;
+}
+static int visual_device(hv_ekf* e, const double* dH, int n, int l, const double* df, const double* dy, double r, double rmseThr,
+                         int mode, double* dResult, int lateH, double* slot = nullptr)
+{
+    EkfUpdateArgs a;
+    int rc = visual_device_args(e, dH, n, l, df, dy, r, rmseThr, mode, lateH, slot, a);
+    if (rc != HV_OK) return rc;
     rc = launch_update(e, a);
     if (rc != HV_OK) return rc;
     if (dResult) HV_CUDA(cudaMemcpyAsync(dResult, e->b.res, 2 * sizeof(double), cudaMemcpyDeviceToDevice, e->ctx->stream));
@@ -921,17 +938,11 @@ static void adopt_second_buffers(hv_ekf* e)
     e->spec.valid = false;
 }
 
-// A run of consecutive check-only VISUAL ops (mode 0) reads the same (m, P) and is therefore issued as ONE launch
-// (one cluster per measurement); with host buffers it is also one H2D copy, one D2H copy and one synchronisation.
-static int flush_checks(hv_ekf* e, const hv_ekf_op* ops, int first, int count, bool host, int* vuStatus, double* chi2, int augDiscarded = -1, bool augSym = false)
+// Argument block of the first of `count` consecutive outlier checks and one batch item per check, with the list's measurement pointers
+static int check_items(hv_ekf* e, const hv_ekf_op* ops, int first, int count, EkfUpdateArgs& a, EkfCheckBatch& b)
 {
-    if (count == 0) return HV_OK;
-    cudaStream_t s = e->ctx->stream;
-    EkfUpdateArgs a; EkfCheckBatch b;
     memset(&b, 0, sizeof(b));
     b.count = count;
-    size_t off = 0;
-    if (host) { int rc = staging_acquire(e); if (rc != HV_OK) return rc; }
     for (int i = 0; i < count; i++) {
         const hv_ekf_op& o = ops[first + i];
         EkfUpdateArgs tmp;
@@ -941,17 +952,41 @@ static int flush_checks(hv_ekf* e, const hv_ekf_op* ops, int first, int count, b
         if (!o.H || !o.f || !o.y) { hv_set_error("hv_ekf_run: op %d: NULL input", first + i); return HV_ERR_INVALID; }
         EkfCheckItem& it = b.it[i];
         it.n = o.n; it.l = o.l; it.Rdiag = tmp.Rdiag; it.chi2Thr = tmp.chi2Thr; it.rmseThr = tmp.rmseThr; it.skipChi2 = tmp.skipChi2;
-        const size_t nl = (size_t)o.n * o.l;
-        if (host) {
+        it.H = o.H; it.f = o.f; it.y = o.y;
+    }
+    return HV_OK;
+}
+// The augmentation that shares the launch of the checks before it: results into the second buffers
+static void fused_augment_args(hv_ekf* e, int discarded, bool symFirst, EkfUpdateArgs& aug)
+{
+    augment_args(e, discarded, symFirst, aug);
+    aug.noiseScale = e->noiseScale; aug.specP = e->b.P2; aug.specM = e->m2;
+}
+
+// A run of consecutive check-only VISUAL ops (mode 0) reads the same (m, P) and is therefore issued as ONE launch
+// (one cluster per measurement); with host buffers it is also one H2D copy, one D2H copy and one synchronisation.
+static int flush_checks(hv_ekf* e, const hv_ekf_op* ops, int first, int count, bool host, int* vuStatus, double* chi2, int augDiscarded = -1, bool augSym = false)
+{
+    if (count == 0) return HV_OK;
+    cudaStream_t s = e->ctx->stream;
+    EkfUpdateArgs a; EkfCheckBatch b;
+    int rci = check_items(e, ops, first, count, a, b);
+    if (rci != HV_OK) return rci;
+    if (host) {
+        int rc = staging_acquire(e);
+        if (rc != HV_OK) return rc;
+        size_t off = 0;
+        for (int i = 0; i < count; i++) {
+            const hv_ekf_op& o = ops[first + i];
+            EkfCheckItem& it = b.it[i];
+            const size_t nl = (size_t)o.n * o.l;
             double* hin = e->h_pin + off;
             memcpy(hin, o.H, nl * sizeof(double)); memcpy(hin + nl, o.f, o.n * sizeof(double)); memcpy(hin + nl + o.n, o.y, o.n * sizeof(double));
             it.H = e->d_in + off; it.f = e->d_in + off + nl; it.y = e->d_in + off + nl + o.n;
             off += nl + 2 * (size_t)o.n;
-        } else { it.H = o.H; it.f = o.f; it.y = o.y; }
-    }
-    if (host) {
+        }
         HV_CUDA(cudaMemcpyAsync(e->d_in, e->h_pin, off * sizeof(double), cudaMemcpyHostToDevice, s));
-        int rc = staging_release(e);
+        rc = staging_release(e);
         if (rc != HV_OK) return rc;
     }
     a.b = e->b; a.noiseScale = e->noiseScale;
@@ -961,8 +996,7 @@ static int flush_checks(hv_ekf* e, const hv_ekf_op* ops, int first, int count, b
     if (augDiscarded >= 0) {
         int rcj = join_side(e);                            // (checks of the previous list read the buffers this augmentation writes)
         if (rcj != HV_OK) return rcj;
-        EkfUpdateArgs aug; augment_args(e, augDiscarded, augSym, aug);
-        aug.noiseScale = e->noiseScale; aug.specP = e->b.P2; aug.specM = e->m2;
+        EkfUpdateArgs aug; fused_augment_args(e, augDiscarded, augSym, aug);
         // HV_EKF_NO_PDL=1 (throughput mode, many sessions per GPU): nothing is launched early or beside the main stream
         static const bool latencyMode = getenv("HV_EKF_NO_PDL") == nullptr;
         if (host || !latencyMode) {
@@ -1017,13 +1051,16 @@ static bool batchable_check(const hv_ekf* e, const hv_ekf_op& o)
            ekf_cluster2_fits(o.n, o.l, e->N, false);
 }
 
+static void note_visual_ops(hv_ekf* e, const hv_ekf_op* ops, int nops)       // which slots of d_opres a list fills (hv_ekf_run_device_results)
+{
+    e->lastVisual.assign(nops, 0);
+    for (int i = 0; i < nops && i < HV_RUN_MAX_OPS; i++) if (ops[i].kind == HV_EKF_OP_VISUAL) e->lastVisual[i] = 1;
+}
+
 static int run_ops(hv_ekf* e, const hv_ekf_op* ops, int nops, bool host, int* vuStatus, double* chi2, double* mOut)
 {
     if (!ops || nops < 0) { hv_set_error("hv_ekf_run: invalid argument"); return HV_ERR_INVALID; }
-    if (!host) {                                                  // which slots of d_opres this list fills (hv_ekf_run_device_results)
-        e->lastVisual.assign(nops, 0);
-        for (int i = 0; i < nops && i < HV_RUN_MAX_OPS; i++) if (ops[i].kind == HV_EKF_OP_VISUAL) e->lastVisual[i] = 1;
-    }
+    if (!host) note_visual_ops(e, ops, nops);
     for (int i = 0; i < nops; i++) {
         const hv_ekf_op& o = ops[i];
         int rc = HV_OK;
@@ -1216,6 +1253,238 @@ int hv_ekf_run_device_results(hv_ekf* e, int nops, int* vuStatus, double* chi2)
         if (vuStatus) vuStatus[i] = (int)hout[4 * i];
         if (chi2) chi2[i] = hout[4 * i + 1];
         if (hout[4 * i + 2] != 0.0) { hv_set_error("hv_ekf_run_device_results: op %d: innovation covariance not positive definite", i); return HV_ERR_STATE; }
+    }
+    return HV_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------- a group of filters
+// hv_ekf_group_run_device: every list is cut into the steps run_ops issues for it -- an IMU burst, one visual update, a run of outlier
+// checks with the augmentation that follows them as one more cluster, an augmentation -- and step k of every filter goes into one launch
+// per kernel, so that a group of filters takes the launches of one. The instances of a step belong to different filters, and step k of
+// a filter is stream-ordered behind its step k - 1.
+struct GroupStep {
+    bool predict = false;
+    EkfPredictArgs p;                       // predict: the burst
+    std::vector<EkfUpdateArgs> u;           // otherwise: one argument block per cluster
+};
+
+static int group_refuse(int rc, int f, int i, const char* what)
+{
+    hv_set_error("hv_ekf_group_run_device: filter %d, op %d: %s", f, i, what);
+    return rc;
+}
+
+// Checks a list against the group's vocabulary (see the header) without changing anything: a dry run of the IMU bookkeeping
+// (predict_bookkeep, the burst length) tells whether each NORMALIZE folds into the sample before it.
+static int group_check_list(hv_ekf* e, const hv_ekf_op* ops, int nops, int f)
+{
+    if (!ops || nops < 0) return group_refuse(HV_ERR_INVALID, f, -1, "NULL list or negative length");
+    bool firstSample = e->firstSample, normed = false;
+    double prevT = e->prevSampleT;
+    int pend = 0;                                        // (the queue is issued before the list: flush_pending)
+    for (int i = 0; i < nops; i++) {
+        const hv_ekf_op& o = ops[i];
+        switch (o.kind) {
+        case HV_EKF_OP_PREDICT: {
+            double dt = 0.0;
+            if (!firstSample) dt = o.t - prevT; else firstSample = false;
+            prevT = o.t;
+            if (dt <= 0.0) break;
+            pend++; normed = false;
+            if (pend >= e->imuBatch) pend = 0;
+        } break;
+        case HV_EKF_OP_NORMALIZE:
+            if (!o.index || pend == 0 || normed) return group_refuse(HV_ERR_UNSUPPORTED, f, i, "NORMALIZE that does not fold into the IMU sample before it");
+            normed = true;
+            break;
+        case HV_EKF_OP_VISUAL: {
+            if (o.mode < 0 || o.mode > 2) return group_refuse(HV_ERR_INVALID, f, i, "bad mode");
+            if (!o.H || !o.f || !o.y) return group_refuse(HV_ERR_INVALID, f, i, "NULL measurement");
+            EkfUpdateArgs a;
+            const int rc = visual_args(e, "hv_ekf_group_run_device", o.n, o.l, o.r, o.rmse_thr, o.mode, a);
+            if (rc != HV_OK) return rc;
+            if (!ekf_cluster2_fits(o.n, o.l, e->N, false)) return group_refuse(HV_ERR_UNSUPPORTED, f, i, "measurement does not fit the cluster kernel whole");
+            pend = 0;
+        } break;
+        case HV_EKF_OP_SYMMETRIZE:
+            if (i + 1 >= nops || ops[i + 1].kind != HV_EKF_OP_AUGMENT) return group_refuse(HV_ERR_UNSUPPORTED, f, i, "SYMMETRIZE not followed by AUGMENT");
+            pend = 0;
+            break;
+        case HV_EKF_OP_AUGMENT: {
+            const int d = o.index == -1 ? e->trail - 1 : o.index;
+            if (d < 0 || d >= e->trail) return group_refuse(HV_ERR_INVALID, f, i, "discarded pose index out of range");
+            if (!ekf_cluster2_fits(EKF_POSE, EKF_CAM + EKF_POSE, e->N, true)) return group_refuse(HV_ERR_UNSUPPORTED, f, i, "augmentation does not fit the cluster kernel");
+            pend = 0;
+        } break;
+        case HV_EKF_OP_UNAUGMENT: return group_refuse(HV_ERR_UNSUPPORTED, f, i, "UNAUGMENT");
+        default: return group_refuse(HV_ERR_INVALID, f, i, "unknown kind");
+        }
+    }
+    return HV_OK;
+}
+
+// What ekf_check_batch_cluster2_kernel makes of (a, b, aug) for its cluster inst
+static EkfUpdateArgs check_instance(const EkfUpdateArgs& a, const EkfCheckBatch& b, const EkfUpdateArgs& aug, int inst)
+{
+    EkfUpdateArgs r = a;
+    if (inst >= b.count) r = aug;
+    else {
+        const EkfCheckItem& it = b.it[inst];
+        r.H = it.H; r.f = it.f; r.y = it.y; r.n = it.n; r.l = it.l;
+        r.Rdiag = it.Rdiag; r.chi2Thr = it.chi2Thr; r.rmseThr = it.rmseThr; r.skipChi2 = it.skipChi2;
+        if (r.sig) r.sig += 4 * inst;
+        if (r.slot) r.slot += 4 * inst;
+    }
+    r.b.res += (size_t)EKF_RES_STRIDE * inst;
+    r.b.cwork += (size_t)inst * 10 * r.b.N * r.b.N;
+    return r;
+}
+
+// The steps of one filter's (checked) list, with the host bookkeeping of every op done as run_ops does it
+static int group_steps(hv_ekf* e, const hv_ekf_op* ops, int nops, std::vector<GroupStep>& st)
+{
+    int rc = flush_pending(e);                           // work queued by earlier calls goes first
+    if (rc == HV_OK) rc = join_side(e);
+    if (rc != HV_OK) return rc;
+    note_visual_ops(e, ops, nops);
+    auto burst = [&]() {
+        if (e->pend.count == 0) return;
+        st.emplace_back();
+        st.back().predict = true;
+        st.back().p = e->pend;
+        predict_settle(e, st.back().p);
+        e->meanIssued = false;
+        e->pend.count = 0;
+    };
+    for (int i = 0; i < nops; i++) {
+        const hv_ekf_op& o = ops[i];
+        if (o.kind == HV_EKF_OP_PREDICT) {
+            predict_bookkeep(e, o.t, o.gyro, o.acc, e->pend);
+            if (e->pend.count >= e->imuBatch) burst();
+            continue;
+        }
+        if (o.kind == HV_EKF_OP_NORMALIZE) { e->pend.s[e->pend.count - 1].normAfter = 1; continue; }
+        burst();
+        st.emplace_back();
+        std::vector<EkfUpdateArgs>& u = st.back().u;
+        if (batchable_check(e, o)) {
+            int cnt = 1;
+            while (i + cnt < nops && cnt < EKF_MAX_BATCH && batchable_check(e, ops[i + cnt])) cnt++;
+            int disc = -1; bool sym = false;
+            const int extra = augment_follows(e, ops, nops, i + cnt, &disc, &sym);
+            EkfUpdateArgs a, aug; EkfCheckBatch b;
+            rc = check_items(e, ops, i, cnt, a, b);
+            if (rc != HV_OK) return rc;
+            a.b = e->b; a.noiseScale = e->noiseScale;
+            if (i + cnt <= HV_RUN_MAX_OPS) a.slot = e->d_opres + 4 * i;
+            if (extra) fused_augment_args(e, disc, sym, aug);
+            else aug = a;
+            for (int j = 0; j < cnt + (extra ? 1 : 0); j++) u.push_back(check_instance(a, b, aug, j));
+            if (extra) { adopt_second_buffers(e); augment_done(e); }
+            i += cnt - 1 + extra;
+        } else if (o.kind == HV_EKF_OP_VISUAL) {
+            EkfUpdateArgs a;
+            rc = visual_device_args(e, o.H, o.n, o.l, o.f, o.y, o.r, o.rmse_thr, o.mode, 0, i < HV_RUN_MAX_OPS ? e->d_opres + 4 * i : nullptr, a);
+            if (rc != HV_OK) return rc;
+            update_settle(e, a);
+            u.push_back(a);
+        } else {                                                  // [SYMMETRIZE,] AUGMENT
+            const bool sym = o.kind == HV_EKF_OP_SYMMETRIZE;
+            const int d = ops[i + sym].index;
+            EkfUpdateArgs a;
+            augment_args(e, d == -1 ? e->trail - 1 : d, sym, a);
+            update_settle(e, a);
+            u.push_back(a);
+            augment_done(e);
+            i += sym;
+        }
+    }
+    return HV_OK;
+}
+
+// Staging of a group call's argument blocks: pinned block `ekfStageNext` of the context's ring (refilled once the copy out of it has
+// completed) and the device block (reused in stream order: the copy into it follows the kernels that read it before)
+static int group_stage(hv_ctx* c, size_t bytes, char** h, char** d, cudaEvent_t* ev)
+{
+    const int i = c->ekfStageNext;
+    if (!c->evEkfStage[i]) HV_CUDA(cudaEventCreateWithFlags(&c->evEkfStage[i], cudaEventDisableTiming));
+    else HV_CUDA(cudaEventSynchronize(c->evEkfStage[i]));
+    size_t cap = 4096;
+    while (cap < bytes) cap *= 2;
+    if (bytes > c->h_ekfStageBytes[i]) {
+        if (c->h_ekfStage[i]) cudaFreeHost(c->h_ekfStage[i]);
+        c->h_ekfStage[i] = nullptr; c->h_ekfStageBytes[i] = 0;
+        HV_CUDA(cudaMallocHost(&c->h_ekfStage[i], cap));
+        c->h_ekfStageBytes[i] = cap;
+    }
+    if (bytes > c->ekfStageBytes) {
+        if (c->d_ekfStage) HV_CUDA(cudaFreeAsync(c->d_ekfStage, c->stream));
+        c->d_ekfStage = nullptr; c->ekfStageBytes = 0;
+        HV_CUDA(cudaMallocAsync(&c->d_ekfStage, cap, c->stream));
+        c->ekfStageBytes = cap;
+    }
+    c->ekfStageNext = (i + 1) % HV_EKF_STAGES;
+    *h = (char*)c->h_ekfStage[i]; *d = (char*)c->d_ekfStage; *ev = c->evEkfStage[i];
+    return HV_OK;
+}
+
+int hv_ekf_group_run_device(hv_ekf* const* ekfs, int count, const hv_ekf_op* const* ops, const int* nops)
+{
+    if (!ekfs || !ops || !nops || count < 1 || count > HV_EKF_GROUP_MAX) {
+        hv_set_error("hv_ekf_group_run_device: NULL array or count %d outside 1..%d", count, HV_EKF_GROUP_MAX); return HV_ERR_INVALID;
+    }
+    for (int f = 0; f < count; f++) {
+        hv_ekf* e = ekfs[f];
+        if (!e) return group_refuse(HV_ERR_INVALID, f, -1, "NULL filter");
+        if (e->ctx != ekfs[0]->ctx) return group_refuse(HV_ERR_INVALID, f, -1, "filter of another context");
+        if (e->N != ekfs[0]->N) return group_refuse(HV_ERR_INVALID, f, -1, "state dimension differs from filter 0");
+        for (int g = 0; g < f; g++) if (ekfs[g] == e) return group_refuse(HV_ERR_INVALID, f, -1, "filter appears twice");
+        const int rc = group_check_list(e, ops[f], nops[f], f);
+        if (rc != HV_OK) return rc;
+    }
+    hv_ctx* c = ekfs[0]->ctx;
+    HV_CUDA(cudaSetDevice(c->device));
+    std::vector<std::vector<GroupStep>> steps(count);
+    size_t nsteps = 0;
+    for (int f = 0; f < count; f++) {
+        const int rc = group_steps(ekfs[f], ops[f], nops[f], steps[f]);
+        if (rc != HV_OK) return rc;
+        nsteps = std::max(nsteps, steps[f].size());
+    }
+    // one predict and one cluster launch per step: their argument arrays one after the other in the staging block
+    struct Launch { size_t off; int count; bool predict; };
+    std::vector<Launch> launches;
+    std::vector<size_t> predOff(nsteps), updOff(nsteps);
+    size_t bytes = 0;
+    auto align16 = [](size_t v) { return (v + 15) & ~(size_t)15; };
+    for (size_t k = 0; k < nsteps; k++) {
+        int np = 0, nu = 0;
+        for (int f = 0; f < count; f++) if (k < steps[f].size()) { if (steps[f][k].predict) np++; else nu += (int)steps[f][k].u.size(); }
+        predOff[k] = bytes;
+        if (np) { launches.push_back({bytes, np, true}); bytes = align16(bytes + np * sizeof(EkfPredictArgs)); }
+        updOff[k] = bytes;
+        if (nu) { launches.push_back({bytes, nu, false}); bytes = align16(bytes + nu * sizeof(EkfUpdateArgs)); }
+    }
+    if (launches.empty()) return HV_OK;
+    char *h = nullptr, *d = nullptr; cudaEvent_t ev = nullptr;
+    int rc = group_stage(c, bytes, &h, &d, &ev);
+    if (rc != HV_OK) return rc;
+    for (size_t k = 0; k < nsteps; k++) {
+        EkfPredictArgs* hp = (EkfPredictArgs*)(h + predOff[k]);
+        EkfUpdateArgs* hu = (EkfUpdateArgs*)(h + updOff[k]);
+        for (int f = 0; f < count; f++) {
+            if (k >= steps[f].size()) continue;
+            const GroupStep& s = steps[f][k];
+            if (s.predict) *hp++ = s.p;
+            else for (const EkfUpdateArgs& a : s.u) *hu++ = a;
+        }
+    }
+    HV_CUDA(cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, c->stream));
+    HV_CUDA(cudaEventRecord(ev, c->stream));
+    for (const Launch& L : launches) {
+        if (L.predict) HV_CUDA(ekf_launch_group_predict((const EkfPredictArgs*)(h + L.off), (const EkfPredictArgs*)(d + L.off), L.count, c->stream));
+        else HV_CUDA(ekf_launch_group_cluster2((const EkfUpdateArgs*)(h + L.off), (const EkfUpdateArgs*)(d + L.off), L.count, c->stream));
+        c->launches++;
     }
     return HV_OK;
 }

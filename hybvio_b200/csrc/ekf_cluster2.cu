@@ -47,6 +47,14 @@ __global__ void __launch_bounds__(EK2_NT) ekf_check_batch_cluster2_kernel(EkfUpd
     ek2_body<false>(a, ek2_sm, cluster);
 }
 
+// Group launch (hv_ekf_group_run_device): cluster i runs args[i], an instance of any filter of the group. The blocks live in device
+// memory (hundreds of clusters do not fit the parameter space); no cluster waits for another, so a grid of many clusters runs in waves.
+__global__ void __launch_bounds__(EK2_NT) ekf_group_cluster2_kernel(const EkfUpdateArgs* __restrict__ args)
+{
+    extern __shared__ __align__(16) double ek2_sm[];
+    ek2_group_body(args, blockIdx.x / EK2_C, ek2_sm, cg::this_cluster());
+}
+
 #define EK2_STATIC_SMEM (sizeof(double) * (2 + EK2_LINV_DOUBLES + 2 + EK2_MAXN) + 256)
 #define EK2_SMEM_LIMIT (227 * 1024)
 
@@ -105,4 +113,13 @@ cudaError_t ekf_launch_check_batch2(const EkfUpdateArgs& a, const EkfCheckBatch&
     for (int i = 0; i < b.count; i++) { const size_t v = ek2_smem_bytes(b.it[i].n, b.it[i].l, a.b.N, false); if (v > smem) smem = v; }
     if (aug) { const size_t v = ek2_smem_bytes(aug->n, aug->l, a.b.N, true); if (v > smem) smem = v; }
     return ek2_launch(ekf_check_batch_cluster2_kernel, b.count + (aug ? 1 : 0), smem, s, a, b, aug ? *aug : a);
+}
+
+cudaError_t ekf_launch_group_cluster2(const EkfUpdateArgs* hArgs, const EkfUpdateArgs* dArgs, int count, cudaStream_t s)
+{
+    static bool seen[64];
+    if (hv_first_use_on_device(seen)) { cudaError_t e = ek2_prepare(ekf_group_cluster2_kernel); if (e != cudaSuccess) return e; }
+    size_t smem = 0;
+    for (int i = 0; i < count; i++) { const size_t v = ek2_smem_bytes(hArgs[i].n, hArgs[i].l, hArgs[i].b.N, hArgs[i].op == EKF_OP_AUGMENT); if (v > smem) smem = v; }
+    return ek2_launch(ekf_group_cluster2_kernel, count, smem, s, dArgs);
 }

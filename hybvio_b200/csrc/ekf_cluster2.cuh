@@ -1031,3 +1031,12 @@ __device__ __forceinline__ void ek2_body(EkfUpdateArgs& a, double* sm, Cluster c
     if (a.bump && c == 0 && tid == 0) *a.bump = *a.bump + 1;          // one writer per grid; kernels of a chain are stream-ordered
     cluster.sync();                                   // nobody may leave while its shared memory can still be read
 }
+
+// Cluster `inst` of a group launch (ekf_group_cluster2_kernel): its own argument block, fully resolved by the host (filter buffers,
+// exchange area, result words, second buffers), read from device memory. Clusters of one launch share nothing.
+template <class Cluster>
+__device__ __forceinline__ void ek2_group_body(const EkfUpdateArgs* __restrict__ args, int inst, double* sm, Cluster cluster)
+{
+    EkfUpdateArgs a = args[inst];
+    ek2_body<false>(a, sm, cluster);
+}

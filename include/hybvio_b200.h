@@ -323,6 +323,27 @@ int hv_ekf_run_device_results(hv_ekf* ekf, int nops, int* vu_status, double* chi
  * round trip, as in the reference interface. m_out (optional, N doubles) receives the final state mean. */
 int hv_ekf_run_host(hv_ekf* ekf, const hv_ekf_op* ops, int nops, int* vu_status, double* chi2, double* m_out);
 
+/* Many independent filters of ONE context stepped together (several sessions per process): for every i, the effect of
+ * hv_ekf_run_device(ekfs[i], ops[i], nops[i]), called for each i in turn -- m, P, the pose count, the time bookkeeping and the result
+ * words hv_ekf_run_device_results(ekfs[i], ...) returns afterwards are bit-identical -- with the launches of one filter: each list is
+ * cut into steps (an IMU burst; one visual update; a run of outlier checks, with the augmentation that follows them as one more
+ * cluster; an augmentation), and step k of every filter goes into one launch per kernel. Asynchronous, on the context's stream; never
+ * on the library's side stream (throughput-mode stream policy); HV_EKF_NO_PDL keeps its meaning. H, f, y are DEVICE pointers and
+ * prepared inputs, as for hv_ekf_run_device. Work queued for a filter by earlier calls is issued first; IMU samples at the end of a
+ * list stay queued, as with hv_ekf_run_device.
+ * The lists may only hold the ops of a device-resident frame:
+ *   - PREDICT, each optionally followed by NORMALIZE with a non-zero index that folds into the sample before it (bursts of up to
+ *     hv_ekf_set_imu_batching samples, 16 by default; a longer run of PREDICTs takes several launches -- a NORMALIZE right after the
+ *     sample that completes a burst, or after a PREDICT that adds no sample, would be a launch of its own and is refused);
+ *   - VISUAL in modes 0, 1, 2 whose measurement fits the cluster kernel whole (n <= 84 at N = 160);
+ *   - AUGMENT, or SYMMETRIZE directly followed by AUGMENT, where the augmentation fits the cluster kernel (N <= 200).
+ * Refused before anything is issued, every filter untouched: HV_ERR_UNSUPPORTED for any other op (UNAUGMENT, a standalone SYMMETRIZE or
+ * NORMALIZE, a measurement or augmentation that does not fit); HV_ERR_INVALID for NULL arrays, a NULL filter, list or measurement
+ * pointer, count outside 1..HV_EKF_GROUP_MAX, filters of different contexts or state dimensions, a filter that appears twice, a bad
+ * mode or shape, an unknown op kind or a discarded-pose index out of range. The caller falls back to per-filter calls. */
+#define HV_EKF_GROUP_MAX 64
+int hv_ekf_group_run_device(hv_ekf* const* ekfs, int count, const hv_ekf_op* const* ops, const int* nops);
+
 int hv_ekf_augment(hv_ekf* ekf, int discarded_pose_index);     /* updateVisualPoseAugmentation (ekf.cpp:848-885) */
 int hv_ekf_unaugment(hv_ekf* ekf);                             /* updateUndoAugmentation (ekf.cpp:888-903) */
 int hv_ekf_symmetrize(hv_ekf* ekf);                            /* maintainPositiveSemiDefinite (ekf.cpp:1059-1067) */
