@@ -181,6 +181,9 @@ def _bind_ekf(lib):
     lib.hv_ekf_run_device_results.argtypes = [c_void_p, c_int, ctypes.POINTER(c_int), ctypes.POINTER(c_double)]
     lib.hv_ekf_run_host.argtypes = [c_void_p, ctypes.POINTER(EkfOp), c_int, ctypes.POINTER(c_int), ctypes.POINTER(c_double), c_void_p]
     lib.hv_ekf_group_run_device.argtypes = [ctypes.POINTER(c_void_p), c_int, ctypes.POINTER(ctypes.POINTER(EkfOp)), ctypes.POINTER(c_int)]
+    lib.hv_ekf_group_visual_tracks.argtypes = [ctypes.POINTER(c_void_p), c_int, ctypes.POINTER(ctypes.POINTER(TrackObs)), ctypes.POINTER(c_int),
+                                               ctypes.POINTER(VisualUpdateParams), ctypes.POINTER(ctypes.POINTER(TrackResult)), ctypes.POINTER(c_int)]
+    lib.hv_ekf_group_visual_tracks.restype = c_int
     lib.hv_ekf_normalize_quaternions.argtypes = [c_void_p, c_int]
     lib.hv_ekf_translate_to.argtypes = [c_void_p, c_void_p]
     lib.hv_ekf_transform_to.argtypes = [c_void_p, c_void_p, c_void_p, c_int]
@@ -216,6 +219,34 @@ def ekf_group_run_device(ekfs, lists):
     O = (ctypes.POINTER(EkfOp) * n)(*[ctypes.cast(ops, ctypes.POINTER(EkfOp)) for ops, _ in pairs])
     K = (c_int * n)(*[k for _, k in pairs])
     check(load().hv_ekf_group_run_device(E, n, O, K), "hv_ekf_group_run_device")
+
+
+def ekf_group_visual_tracks(ekfs, tracks_per_filter, params_per_filter):
+    """hv_ekf_group_visual_tracks: the visual-update chains of several filters of one context with the launches of one chain.
+    tracks_per_filter[i]: filter i's tracks, as for Ekf.visual_tracks (may be empty); params_per_filter[i]: a VisualUpdateParams or a
+    dict of Ekf.visual_tracks' keyword arguments (chi_outlier_r, visual_r, track_rmse_threshold, max_successful_updates, lookahead).
+    Returns, per filter, what Ekf.visual_tracks returns: (list of dicts per track, number of successful updates). Raises HvError on a
+    refusal (the filters are then untouched) and on a numerical failure."""
+    n = len(ekfs)
+    packed = [ekfs[i]._pack_tracks(t) if len(t) else (None, None) for i, t in enumerate(tracks_per_filter)]
+    outs = [(TrackResult * len(t))() if len(t) else None for t in tracks_per_filter]
+    E = (c_void_p * n)(*[e.h for e in ekfs])
+    T = (ctypes.POINTER(TrackObs) * n)(*[ctypes.cast(obs, ctypes.POINTER(TrackObs)) if obs is not None else None for obs, _ in packed])
+    K = (c_int * n)(*[len(t) for t in tracks_per_filter])
+    P = (VisualUpdateParams * n)(*[p if isinstance(p, VisualUpdateParams) else _visual_params(**p) for p in params_per_filter])
+    O = (ctypes.POINTER(TrackResult) * n)(*[ctypes.cast(o, ctypes.POINTER(TrackResult)) if o is not None else None for o in outs])
+    succ = (c_int * n)()
+    check(load().hv_ekf_group_visual_tracks(E, n, T, K, P, O, succ), "hv_ekf_group_visual_tracks")
+    return [(_track_results(o) if o is not None else [], succ[i]) for i, o in enumerate(outs)]
+
+
+def _visual_params(chi_outlier_r, visual_r, track_rmse_threshold=-1.0, max_successful_updates=5, lookahead=0):
+    return VisualUpdateParams(chi_outlier_r, track_rmse_threshold, visual_r, max_successful_updates, lookahead)
+
+
+def _track_results(out):
+    return [{"tri_status": o.triangulator_status, "vu_status": o.prepare_vu_status, "outlier_status": o.outlier_status, "updated": bool(o.updated),
+             "chi2": o.chi2, "pf": np.array(o.pf[:]), "depth": o.depth} for o in out]
 
 
 class Context:
@@ -600,13 +631,11 @@ class Ekf:
         """hv_ekf_visual_tracks: the per-track model -> check -> update chain with the control flow on the device.
         Returns (list of dicts per track, number of successful updates)."""
         obs, keep = self._pack_tracks(tracks)
-        prm = VisualUpdateParams(chi_outlier_r, track_rmse_threshold, visual_r, max_successful_updates, lookahead)
+        prm = _visual_params(chi_outlier_r, visual_r, track_rmse_threshold, max_successful_updates, lookahead)
         out = (TrackResult * len(tracks))()
         succ = c_int(0)
         check(self.lib.hv_ekf_visual_tracks(self.h, obs, len(tracks), ctypes.byref(prm), out, ctypes.byref(succ)), "hv_ekf_visual_tracks")
-        res = [{"tri_status": o.triangulator_status, "vu_status": o.prepare_vu_status, "outlier_status": o.outlier_status, "updated": bool(o.updated),
-                "chi2": o.chi2, "pf": np.array(o.pf[:]), "depth": o.depth} for o in out]
-        return res, succ.value
+        return _track_results(out), succ.value
 
     def track_models_time(self, reps=50):
         """Average device time (us) of the kernel of the last track_models call."""

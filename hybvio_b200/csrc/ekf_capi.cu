@@ -1556,15 +1556,13 @@ static int tm_reserve(TrackModels* t, int n)
     return HV_OK;
 }
 
-// Validates a batch of tracks, packs it into the pinned block, enqueues the H2D copies and fills the kernel arguments
-// (everything except ntracks / trackOffset / counter).
-static int tm_submit(hv_ekf* e, const char* who, const hv_track_obs* tracks, int ntracks, TmArgs& a)
+// The checks of tm_submit: a camera model, and well-formed tracks
+static int tm_validate(const hv_ekf* e, const char* who, const hv_track_obs* tracks, int ntracks)
 {
-    TrackModels* t = e->tm;
+    const TrackModels* t = e->tm;
     if (!t || !t->camSet) { hv_set_error("%s: hv_ekf_set_camera_model has not been called", who); return HV_ERR_STATE; }
     if (!tracks || ntracks < 1) { hv_set_error("%s: invalid argument", who); return HV_ERR_INVALID; }
     const int maxIndex = e->trail < TM_MAXPOSE - 1 ? e->trail : TM_MAXPOSE - 1;
-    const int ncam = t->cam.use_stereo ? 2 : 1;
     for (int k = 0; k < ntracks; k++) {
         const hv_track_obs& o = tracks[k];
         if (o.npose < 2 || o.npose > TM_MAXPOSE || !o.pose_trail_index || !o.ip || !o.velocities) {
@@ -1575,7 +1573,18 @@ static int tm_submit(hv_ekf* e, const char* who, const hv_track_obs* tracks, int
                 hv_set_error("%s: track %d: pose index %d outside 0..%d", who, k, o.pose_trail_index[i], maxIndex); return HV_ERR_INVALID;
             }
     }
-    int rc = tm_reserve(t, ntracks);
+    return HV_OK;
+}
+
+// Validates a batch of tracks, packs it into the pinned block, enqueues the H2D copies and fills the kernel arguments
+// (everything except ntracks / trackOffset / counter).
+static int tm_submit(hv_ekf* e, const char* who, const hv_track_obs* tracks, int ntracks, TmArgs& a)
+{
+    int rc = tm_validate(e, who, tracks, ntracks);
+    if (rc != HV_OK) return rc;
+    TrackModels* t = e->tm;
+    const int ncam = t->cam.use_stereo ? 2 : 1;
+    rc = tm_reserve(t, ntracks);
     if (rc != HV_OK) return rc;
     cudaStream_t s = e->ctx->stream;
     // pack: the block layout is fixed by the capacity, so that the live ranges are three contiguous copies
@@ -1666,108 +1675,301 @@ static int track_cols(const hv_track_obs& o)
 // The per-track loop of Session::trackerVisualUpdate (src/odometry/backend.cpp:1012-1252, per-track mode) as ONE stream-ordered
 // chain with the control flow on the device: for every track  model(state) -> outlier check -> update if inlier,  each kernel
 // gated by words the previous ones wrote (model valid, fewer than max_successful_updates so far, check said INLIER). The host
-// synchronises once per `lookahead` tracks instead of twice per track.
-int hv_ekf_visual_tracks(hv_ekf* e, const hv_track_obs* tracks, int ntracks, const hv_visual_update_params* p, hv_track_result* out,
-                         int* successfulUpdates)
+// synchronises once per `lookahead` tracks instead of twice per track. A chain belongs to one filter: hv_ekf_visual_tracks issues it
+// alone, hv_ekf_group_visual_tracks track by track beside the chains of other filters; both through the chain_* functions below.
+struct VisualChain {
+    const hv_track_obs* tracks = nullptr;
+    int ntracks = 0;
+    hv_visual_update_params p;
+    TmArgs base;                            // the model arguments of the whole batch (tm_submit)
+    std::vector<int> chunkRows;             // per track: 0 = the cluster kernel on the whole measurement, else its row-chunked form
+    int* d_counter = nullptr;               // control block (TrackModels::d_ctl): success counter, then per track the result slots of
+    double* d_slots = nullptr;              // check (4 doubles) and update (4 doubles)
+    int maxSucc = 0, step = 0;              // step: tracks per host synchronisation
+    bool fused = false;                     // check and update of a track in ONE kernel
+    int issued = 0, succ = 0;               // tracks issued and successful updates, as of the last synchronisation
+};
+
+// Every track's kernel form up front: the cluster kernel on the whole measurement, or its row-chunked form beside the resident P
+// blocks; a chain that contains a track neither fits is refused before anything is issued (tm_submit reports malformed tracks)
+static int chain_forms(const hv_ekf* e, const char* who, const hv_track_obs* tracks, int ntracks, std::vector<int>& chunkRows)
 {
-    EKF_ENTER(e, "hv_ekf_visual_tracks");
-    const char* who = "hv_ekf_visual_tracks";
-    if (!p || !out) { hv_set_error("%s: invalid argument", who); return HV_ERR_INVALID; }
-    // Every track's kernel form up front: the cluster kernel on the whole measurement, or its row-chunked form beside the resident P
-    // blocks; a chain that contains a track neither fits is refused before anything is issued (tm_submit reports malformed tracks)
-    std::vector<int> chunkRows(ntracks > 0 ? ntracks : 0, 0);
-    if (e->tm && e->tm->camSet && tracks) {
-        const int ncam = e->tm->cam.use_stereo ? 2 : 1;
-        for (int k = 0; k < ntracks; k++) {
-            const hv_track_obs& o = tracks[k];
-            if (o.npose < 2 || o.npose > TM_MAXPOSE || !o.pose_trail_index) continue;
-            const int n = 2 * o.npose * ncam, l = track_cols(o);
-            if (ekf_cluster2_fits(n, l, e->N, false)) continue;
-            chunkRows[k] = ekf_cluster2_chunk_rows(n, l, e->N);
-            if (chunkRows[k] == 0) {
-                hv_set_error("%s: track %d (n=%d, l=%d): state dimension %d too large for the cluster kernel, even in row chunks", who, k, n, l, e->N);
-                return HV_ERR_UNSUPPORTED;
-            }
+    chunkRows.assign(ntracks > 0 ? ntracks : 0, 0);
+    if (!e->tm || !e->tm->camSet || !tracks) return HV_OK;
+    const int ncam = e->tm->cam.use_stereo ? 2 : 1;
+    for (int k = 0; k < ntracks; k++) {
+        const hv_track_obs& o = tracks[k];
+        if (o.npose < 2 || o.npose > TM_MAXPOSE || !o.pose_trail_index) continue;
+        const int n = 2 * o.npose * ncam, l = track_cols(o);
+        if (ekf_cluster2_fits(n, l, e->N, false)) continue;
+        chunkRows[k] = ekf_cluster2_chunk_rows(n, l, e->N);
+        if (chunkRows[k] == 0) {
+            hv_set_error("%s: track %d (n=%d, l=%d): state dimension %d too large for the cluster kernel, even in row chunks", who, k, n, l, e->N);
+            return HV_ERR_UNSUPPORTED;
         }
     }
-    TmArgs base;
-    int rc = tm_submit(e, who, tracks, ntracks, base);
+    return HV_OK;
+}
+
+// What precedes the chain's first kernel: the tracks' inputs on the device (tm_submit) and the success counter reset
+static int chain_begin(hv_ekf* e, const char* who, const hv_track_obs* tracks, int ntracks, const hv_visual_update_params* p, VisualChain& ch)
+{
+    int rc = chain_forms(e, who, tracks, ntracks, ch.chunkRows);
+    if (rc != HV_OK) return rc;
+    rc = tm_submit(e, who, tracks, ntracks, ch.base);
     if (rc != HV_OK) return rc;
     TrackModels* t = e->tm;
-    cudaStream_t s = e->ctx->stream;
     if (t->ctlCap < t->cap) {
         cudaFree(t->d_ctl); cudaFreeHost(t->h_ctl); t->d_ctl = t->h_ctl = nullptr; t->ctlCap = 0;
         HV_CUDA(cudaMalloc(&t->d_ctl, TrackModels::ctlBytes(t->cap)));
         HV_CUDA(cudaHostAlloc(&t->h_ctl, TrackModels::ctlBytes(t->cap), cudaHostAllocDefault));
         t->ctlCap = t->cap;
     }
-    int* d_counter = (int*)t->d_ctl;
-    double* d_slots = (double*)(t->d_ctl + 16);                       // per track: check (4 doubles), update (4 doubles)
-    HV_CUDA(cudaMemsetAsync(t->d_ctl, 0, 16, s));
-    const int maxSucc = p->max_successful_updates > 0 ? p->max_successful_updates : 0x7fffffff;
-    const int ncam = t->cam.use_stereo ? 2 : 1;
-    const int step = p->lookahead > 0 ? p->lookahead : ntracks;
+    ch.d_counter = (int*)t->d_ctl;
+    ch.d_slots = (double*)(t->d_ctl + 16);
+    HV_CUDA(cudaMemsetAsync(t->d_ctl, 0, 16, e->ctx->stream));
+    ch.tracks = tracks; ch.ntracks = ntracks; ch.p = *p;
+    ch.maxSucc = p->max_successful_updates > 0 ? p->max_successful_updates : 0x7fffffff;
+    ch.step = p->lookahead > 0 ? p->lookahead : ntracks;
     // check and update of a track in ONE kernel (S0 = H P H' formed once, factorised with each of the two R): one launch
     // fewer per track than separate gated check / update launches.
-    const bool fused = p->chi_outlier_r >= 0.0 && p->visual_r > 0.0;
-    int issued = 0, succ = 0;
-    while (issued < ntracks && succ < maxSucc) {
-        const int first = issued, count = ntracks - issued < step ? ntracks - issued : step;
-        for (int k = first; k < first + count; k++) {
-            TmArgs a = base;
-            a.ntracks = 1; a.trackOffset = k; a.counter = d_counter; a.counterMax = maxSucc;
-            a.pdl = k > first ? 1 : 0;                                // behind a cluster kernel of this chain: overlap the launch with its tail
-            HV_CUDA(tm_launch(a, s));
-            e->ctx->launches++;
-            const hv_track_obs& o = tracks[k];
-            const int n = 2 * o.npose * ncam, l = track_cols(o);
-            double* slotC = d_slots + 8 * (size_t)k;
-            EkfUpdateArgs c;
-            rc = visual_args(e, who, n, l, p->chi_outlier_r, p->track_rmse_threshold, fused ? EKF_MODE_CHECK_UPDATE : EKF_MODE_CHECK, c);
-            if (rc != HV_OK) return rc;
-            c.H = t->d_H + (size_t)k * TrackModels::hStride(); c.f = t->d_f + (size_t)k * 2 * TM_MAXOBS; c.y = base.ip + (size_t)k * 2 * TM_MAXOBS;
-            c.gateI = base.status + 4 * (size_t)k + 1; c.gateIExpect = 0; c.counter = d_counter; c.counterMax = maxSucc; c.slot = slotC; c.lateH = 1;
-            if (fused) { c.Rdiag2 = (p->visual_r * p->visual_r) * e->noiseScale; c.bump = d_counter; }      // check with chi_outlier_r, update with visual_r, one kernel
-            c.rowChunk = chunkRows[k];
-            rc = launch_update(e, c);
-            if (rc != HV_OK) return rc;
-            if (fused) continue;
-            EkfUpdateArgs u;
-            rc = visual_args(e, who, n, l, p->visual_r, -1.0, EKF_MODE_UPDATE, u);
-            if (rc != HV_OK) return rc;
-            u.H = c.H; u.f = c.f; u.y = c.y;
-            u.gateD = slotC; u.gateDExpect = 0.0;                     // VuOutlierStatus::INLIER
-            u.bump = d_counter; u.slot = slotC + 4; u.lateH = 1; u.rowChunk = chunkRows[k];
-            rc = launch_update(e, u);
-            if (rc != HV_OK) return rc;
-        }
-        rc = tm_fetch(e, first, count);
-        if (rc != HV_OK) return rc;
-        HV_CUDA(cudaMemcpyAsync(t->h_ctl, t->d_ctl, 16, cudaMemcpyDeviceToHost, s));
-        HV_CUDA(cudaMemcpyAsync(t->h_ctl + 16 + 64 * (size_t)first, t->d_ctl + 16 + 64 * (size_t)first, 64 * (size_t)count, cudaMemcpyDeviceToHost, s));
-        HV_CUDA(cudaStreamSynchronize(s));
-        succ = *(const int*)t->h_ctl;
-        issued += count;
-    }
-    const double* slots = (const double*)(t->h_ctl + 16);
+    ch.fused = p->chi_outlier_r >= 0.0 && p->visual_r > 0.0;
+    ch.issued = ch.succ = 0;
+    return HV_OK;
+}
+
+static bool chain_open(const VisualChain& ch) { return ch.issued < ch.ntracks && ch.succ < ch.maxSucc; }      // another window to issue
+static int chain_window(const VisualChain& ch) { return std::min(ch.step, ch.ntracks - ch.issued); }         // its length
+
+// The argument blocks of track k, settled for issue in this order: the model m, the check (fused: check + update) c and, unless the
+// chain is fused, the update u. pdl: m follows a kernel of the chain on the stream.
+static int chain_track(hv_ekf* e, const char* who, const VisualChain& ch, int k, int pdl, TmArgs& m, EkfUpdateArgs& c, EkfUpdateArgs& u)
+{
+    m = ch.base;
+    m.ntracks = 1; m.trackOffset = k; m.counter = ch.d_counter; m.counterMax = ch.maxSucc; m.pdl = pdl;
+    const TrackModels* t = e->tm;
+    const hv_track_obs& o = ch.tracks[k];
+    const int n = 2 * o.npose * (t->cam.use_stereo ? 2 : 1), l = track_cols(o);
+    double* slotC = ch.d_slots + 8 * (size_t)k;
+    int rc = visual_args(e, who, n, l, ch.p.chi_outlier_r, ch.p.track_rmse_threshold, ch.fused ? EKF_MODE_CHECK_UPDATE : EKF_MODE_CHECK, c);
+    if (rc != HV_OK) return rc;
+    c.H = t->d_H + (size_t)k * TrackModels::hStride(); c.f = t->d_f + (size_t)k * 2 * TM_MAXOBS; c.y = ch.base.ip + (size_t)k * 2 * TM_MAXOBS;
+    c.gateI = ch.base.status + 4 * (size_t)k + 1; c.gateIExpect = 0; c.counter = ch.d_counter; c.counterMax = ch.maxSucc; c.slot = slotC; c.lateH = 1;
+    if (ch.fused) { c.Rdiag2 = (ch.p.visual_r * ch.p.visual_r) * e->noiseScale; c.bump = ch.d_counter; }      // check with chi_outlier_r, update with visual_r, one kernel
+    c.rowChunk = ch.chunkRows[k];
+    update_settle(e, c);
+    if (ch.fused) return HV_OK;
+    rc = visual_args(e, who, n, l, ch.p.visual_r, -1.0, EKF_MODE_UPDATE, u);
+    if (rc != HV_OK) return rc;
+    u.H = c.H; u.f = c.f; u.y = c.y;
+    u.gateD = slotC; u.gateDExpect = 0.0;                     // VuOutlierStatus::INLIER
+    u.bump = ch.d_counter; u.slot = slotC + 4; u.lateH = 1; u.rowChunk = ch.chunkRows[k];
+    update_settle(e, u);
+    return HV_OK;
+}
+
+// D2H copies (asynchronous) of what the window [ch.issued, ch.issued + count) wrote: model words, success counter, result slots
+static int chain_fetch(hv_ekf* e, const VisualChain& ch, int count)
+{
+    const int first = ch.issued;
+    int rc = tm_fetch(e, first, count);
+    if (rc != HV_OK) return rc;
+    TrackModels* t = e->tm;
+    cudaStream_t s = e->ctx->stream;
+    HV_CUDA(cudaMemcpyAsync(t->h_ctl, t->d_ctl, 16, cudaMemcpyDeviceToHost, s));
+    HV_CUDA(cudaMemcpyAsync(t->h_ctl + 16 + 64 * (size_t)first, t->d_ctl + 16 + 64 * (size_t)first, 64 * (size_t)count, cudaMemcpyDeviceToHost, s));
+    return HV_OK;
+}
+// after the synchronisation behind chain_fetch(ch, count)
+static void chain_synced(const hv_ekf* e, VisualChain& ch, int count)
+{
+    ch.succ = *(const int*)e->tm->h_ctl;
+    ch.issued += count;
+}
+
+// Every track's record (tracks the chain never issued: not attempted) and the number of successful updates
+static int chain_results(const hv_ekf* e, const char* who, const VisualChain& ch, hv_track_result* out, int* successfulUpdates)
+{
+    const double* slots = (const double*)(e->tm->h_ctl + 16);
     bool numeric = false;
-    for (int k = 0; k < ntracks; k++) {
+    for (int k = 0; k < ch.ntracks; k++) {
         hv_track_result& o = out[k];
         memset(&o, 0, sizeof(o));
-        if (k >= issued) { o.triangulator_status = TM_SKIPPED; o.prepare_vu_status = TM_VU_NOT_RUN; o.outlier_status = 1; continue; }
+        if (k >= ch.issued) { o.triangulator_status = TM_SKIPPED; o.prepare_vu_status = TM_VU_NOT_RUN; o.outlier_status = 1; continue; }
         hv_track_model mdl;
-        tm_result(e, base, k, mdl);
+        tm_result(e, ch.base, k, mdl);
         o.triangulator_status = mdl.triangulator_status; o.prepare_vu_status = mdl.prepare_vu_status;
         for (int r = 0; r < 3; r++) o.pf[r] = mdl.pf[r];
         o.depth = mdl.depth;
         const double* sc = slots + 8 * (size_t)k;
         o.outlier_status = (int)sc[0]; o.chi2 = sc[1];
-        o.updated = fused ? ((sc[0] == 0.0 && sc[2] == 0.0) ? 1 : 0) : ((sc[0] == 0.0 && sc[4] == 0.0 && sc[6] == 0.0) ? 1 : 0);
-        numeric = numeric || sc[2] != 0.0 || (!fused && sc[6] != 0.0);
+        o.updated = ch.fused ? ((sc[0] == 0.0 && sc[2] == 0.0) ? 1 : 0) : ((sc[0] == 0.0 && sc[4] == 0.0 && sc[6] == 0.0) ? 1 : 0);
+        numeric = numeric || sc[2] != 0.0 || (!ch.fused && sc[6] != 0.0);
     }
-    if (successfulUpdates) *successfulUpdates = succ;
+    if (successfulUpdates) *successfulUpdates = ch.succ;
     if (numeric) { hv_set_error("%s: innovation covariance not positive definite", who); return HV_ERR_STATE; }
     return HV_OK;
+}
+
+int hv_ekf_visual_tracks(hv_ekf* e, const hv_track_obs* tracks, int ntracks, const hv_visual_update_params* p, hv_track_result* out,
+                         int* successfulUpdates)
+{
+    EKF_ENTER(e, "hv_ekf_visual_tracks");
+    const char* who = "hv_ekf_visual_tracks";
+    if (!p || !out) { hv_set_error("%s: invalid argument", who); return HV_ERR_INVALID; }
+    VisualChain ch;
+    int rc = chain_begin(e, who, tracks, ntracks, p, ch);
+    if (rc != HV_OK) return rc;
+    cudaStream_t s = e->ctx->stream;
+    while (chain_open(ch)) {
+        const int first = ch.issued, count = chain_window(ch);
+        for (int k = first; k < first + count; k++) {
+            TmArgs m; EkfUpdateArgs c, u;
+            rc = chain_track(e, who, ch, k, k > first ? 1 : 0, m, c, u);     // pdl: behind a cluster kernel of this chain, overlap the launch with its tail
+            if (rc != HV_OK) return rc;
+            HV_CUDA(tm_launch(m, s));
+            e->ctx->launches++;
+            HV_CUDA(ekf_launch_update(c, s));
+            e->ctx->launches++;
+            if (ch.fused) continue;
+            HV_CUDA(ekf_launch_update(u, s));
+            e->ctx->launches++;
+        }
+        rc = chain_fetch(e, ch, count);
+        if (rc != HV_OK) return rc;
+        HV_CUDA(cudaStreamSynchronize(s));
+        chain_synced(e, ch, count);
+    }
+    return chain_results(e, who, ch, out, successfulUpdates);
+}
+
+// ---------------------------------------------------------------------------------------------------- visual-update chains of a group
+// hv_ekf_group_visual_tracks: step j issues the next track of every chain that has one left in its current window -- one launch of
+// hv_track_model_group_kernel (a CTA per filter), one of ekf_group_cluster2_kernel (a cluster per filter: the check + update, or the check
+// of a chain in the separate form) and, if a chain of the step uses the separate form, one more for the updates of those chains. Each
+// chain keeps its own windows of `lookahead` tracks; the host synchronises, once for all, when a chain has reached the end of a window
+// after which it may have to stop (a window that ends the list needs no decision).
+int hv_ekf_group_visual_tracks(hv_ekf* const* ekfs, int count, const hv_track_obs* const* tracks, const int* ntracks,
+                               const hv_visual_update_params* params, hv_track_result* const* out, int* successfulUpdates)
+{
+    const char* who = "hv_ekf_group_visual_tracks";
+    if (!ekfs || !tracks || !ntracks || !params || !out || count < 1 || count > HV_EKF_GROUP_MAX) {
+        hv_set_error("%s: NULL array or count %d outside 1..%d", who, count, HV_EKF_GROUP_MAX); return HV_ERR_INVALID;
+    }
+    // everything that can be refused, before anything is issued
+    std::vector<std::string> whoF(count);               // "hv_ekf_group_visual_tracks: filter f" (error messages name the filter)
+    for (int f = 0; f < count; f++) {
+        char buf[64];
+        snprintf(buf, sizeof(buf), "%s: filter %d", who, f);
+        whoF[f] = buf;
+        const char* wf = whoF[f].c_str();
+        hv_ekf* e = ekfs[f];
+        if (!e) { hv_set_error("%s: NULL filter", wf); return HV_ERR_INVALID; }
+        if (e->ctx != ekfs[0]->ctx) { hv_set_error("%s: filter of another context", wf); return HV_ERR_INVALID; }
+        if (e->N != ekfs[0]->N) { hv_set_error("%s: state dimension differs from filter 0", wf); return HV_ERR_INVALID; }
+        for (int g = 0; g < f; g++) if (ekfs[g] == e) { hv_set_error("%s: filter appears twice", wf); return HV_ERR_INVALID; }
+        if (ntracks[f] < 0 || (ntracks[f] > 0 && (!tracks[f] || !out[f]))) { hv_set_error("%s: negative track count, or NULL tracks or results", wf); return HV_ERR_INVALID; }
+        if (!e->tm || !e->tm->camSet) { hv_set_error("%s: hv_ekf_set_camera_model has not been called", wf); return HV_ERR_STATE; }
+        if (ntracks[f] == 0) continue;
+        int rc = tm_validate(e, wf, tracks[f], ntracks[f]);
+        if (rc != HV_OK) return rc;
+        const int ncam = e->tm->cam.use_stereo ? 2 : 1;
+        for (int k = 0; k < ntracks[f]; k++) {
+            const hv_track_obs& o = tracks[f][k];
+            const int n = 2 * o.npose * ncam, l = track_cols(o);
+            EkfUpdateArgs a;
+            rc = visual_args(e, wf, n, l, params[f].chi_outlier_r, params[f].track_rmse_threshold, EKF_MODE_CHECK, a);
+            if (rc != HV_OK) return rc;
+            if (!ekf_cluster2_fits(n, l, e->N, false)) {
+                hv_set_error("%s, track %d (n=%d, l=%d): the measurement does not fit the cluster kernel whole at N = %d (the group has no row-chunked form)",
+                             wf, k, n, l, e->N);
+                return HV_ERR_UNSUPPORTED;
+            }
+        }
+    }
+    hv_ctx* c = ekfs[0]->ctx;
+    HV_CUDA(cudaSetDevice(c->device));
+    std::vector<VisualChain> ch(count);
+    std::vector<int> next(count, 0), winEnd(count, 0);  // per chain: the next track to issue, the end of its current window
+    for (int f = 0; f < count; f++) {
+        if (ntracks[f] == 0) continue;
+        int rc = flush_pending(ekfs[f]);                 // (EKF_ENTER: work queued by earlier calls goes first)
+        if (rc == HV_OK) rc = chain_begin(ekfs[f], whoF[f].c_str(), tracks[f], ntracks[f], &params[f], ch[f]);
+        if (rc != HV_OK) return rc;
+        winEnd[f] = chain_window(ch[f]);
+    }
+    auto align16 = [](size_t v) { return (v + 15) & ~(size_t)15; };
+    for (;;) {
+        // steps up to the first window end that needs a decision; if none does, up to the end of the longest chain
+        int D = 0x7fffffff, longest = 0;
+        for (int f = 0; f < count; f++) {
+            const int left = winEnd[f] - next[f];
+            if (left <= 0) continue;
+            longest = std::max(longest, left);
+            if (winEnd[f] < ntracks[f]) D = std::min(D, left);
+        }
+        if (longest == 0) break;
+        if (D == 0x7fffffff) D = longest;
+        // the argument blocks of these D steps: per step the model blocks, the cluster blocks, the update blocks, in one staging block
+        std::vector<std::vector<TmArgs>> M(D);
+        std::vector<std::vector<EkfUpdateArgs>> C(D), U(D);
+        for (int j = 0; j < D; j++)
+            for (int f = 0; f < count; f++) {
+                if (next[f] + j >= winEnd[f]) continue;
+                TmArgs m; EkfUpdateArgs cu, u;
+                const int rc = chain_track(ekfs[f], whoF[f].c_str(), ch[f], next[f] + j, j > 0 ? 1 : 0, m, cu, u);
+                if (rc != HV_OK) return rc;
+                M[j].push_back(m); C[j].push_back(cu);
+                if (!ch[f].fused) U[j].push_back(u);
+            }
+        std::vector<size_t> offM(D), offC(D), offU(D);
+        size_t bytes = 0;
+        for (int j = 0; j < D; j++) {
+            offM[j] = bytes; bytes = align16(bytes + M[j].size() * sizeof(TmArgs));
+            offC[j] = bytes; bytes = align16(bytes + C[j].size() * sizeof(EkfUpdateArgs));
+            offU[j] = bytes; bytes = align16(bytes + U[j].size() * sizeof(EkfUpdateArgs));
+        }
+        char *h = nullptr, *d = nullptr; cudaEvent_t ev = nullptr;
+        int rc = group_stage(c, bytes, &h, &d, &ev);
+        if (rc != HV_OK) return rc;
+        for (int j = 0; j < D; j++) {
+            memcpy(h + offM[j], M[j].data(), M[j].size() * sizeof(TmArgs));
+            memcpy(h + offC[j], C[j].data(), C[j].size() * sizeof(EkfUpdateArgs));
+            if (!U[j].empty()) memcpy(h + offU[j], U[j].data(), U[j].size() * sizeof(EkfUpdateArgs));
+        }
+        HV_CUDA(cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, c->stream));
+        HV_CUDA(cudaEventRecord(ev, c->stream));
+        for (int j = 0; j < D; j++) {
+            HV_CUDA(tm_launch_group((const TmArgs*)(h + offM[j]), (const TmArgs*)(d + offM[j]), (int)M[j].size(), c->stream));
+            HV_CUDA(ekf_launch_group_cluster2((const EkfUpdateArgs*)(h + offC[j]), (const EkfUpdateArgs*)(d + offC[j]), (int)C[j].size(), c->stream));
+            c->launches += 2;
+            if (U[j].empty()) continue;
+            HV_CUDA(ekf_launch_group_cluster2((const EkfUpdateArgs*)(h + offU[j]), (const EkfUpdateArgs*)(d + offU[j]), (int)U[j].size(), c->stream));
+            c->launches++;
+        }
+        // the chains that have reached the end of a window hand their results back: one synchronisation for all of them
+        std::vector<int> ended;
+        for (int f = 0; f < count; f++) {
+            if (next[f] >= winEnd[f]) continue;
+            next[f] = std::min(next[f] + D, winEnd[f]);
+            if (next[f] < winEnd[f]) continue;
+            ended.push_back(f);
+            rc = chain_fetch(ekfs[f], ch[f], winEnd[f] - ch[f].issued);
+            if (rc != HV_OK) return rc;
+        }
+        HV_CUDA(cudaStreamSynchronize(c->stream));
+        for (int f : ended) {
+            chain_synced(ekfs[f], ch[f], winEnd[f] - ch[f].issued);
+            if (chain_open(ch[f])) winEnd[f] = ch[f].issued + chain_window(ch[f]);
+        }
+    }
+    int rc = HV_OK;
+    for (int f = count - 1; f >= 0; f--) {               // (in reverse: the error message names the first filter whose update failed)
+        if (ntracks[f] == 0) { if (successfulUpdates) successfulUpdates[f] = 0; continue; }
+        const int rcf = chain_results(ekfs[f], whoF[f].c_str(), ch[f], out[f], successfulUpdates ? successfulUpdates + f : nullptr);
+        if (rcf != HV_OK) rc = rcf;
+    }
+    return rc;
 }
 
 // Outlier check / update on a measurement model that is already on the device (hv_ekf_track_models): same launch and result

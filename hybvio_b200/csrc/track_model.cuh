@@ -256,13 +256,14 @@ __device__ __forceinline__ int tm_pos_index(int i) { return i == 0 ? TM_POS : TM
 __device__ __forceinline__ int tm_ori_index(int i) { return i == 0 ? TM_ORI : TM_CAM + 7 * (i - 1) + 3; }
 
 // ---------------------------------------------------------------------------------------------------- the kernel body
-__device__ __forceinline__ void tm_body(const TmArgs& a, double* sm)
+// block: the CTA's index among the tracks of a.  The CTA handles track block + a.trackOffset.
+__device__ __forceinline__ void tm_body(const TmArgs& a, double* sm, int block)
 {
     __shared__ int s_colmap[TM_MAXN], s_code[TM_MAXOBS];
     // NT threads (a multiple of 32, >= 256: the 4-lane reductions of stage C4 address 63 x 4 threads): TM_NT in its own kernel, the
     // 512 threads of a cluster CTA when the persistent chain kernel runs the model in its CTA 0
     const int NT = (int)blockDim.x;
-    const int tid = threadIdx.x, trk = blockIdx.x + a.trackOffset, lane = tid & 31, wrp = tid >> 5;
+    const int tid = threadIdx.x, trk = block + a.trackOffset, lane = tid & 31, wrp = tid >> 5;
 #ifndef HV_EMU
     if (a.pdl) {        // the next kernel of the chain may be scheduled now (it reads nothing of ours before its own wait); then wait for our predecessor
         asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
@@ -613,3 +614,9 @@ __device__ __forceinline__ void tm_body(const TmArgs& a, double* sm)
         }
     }
 }
+// CTA blockIdx.x of a batch (the emulator drivers of tests/emu call this form)
+__device__ __forceinline__ void tm_body(const TmArgs& a, double* sm) { tm_body(a, sm, (int)blockIdx.x); }
+
+// CTA `inst` of a group launch (hv_track_model_group_kernel): the first track of its own argument block args[inst], one filter's
+// chain step, read from device memory
+__device__ __forceinline__ void tm_group_body(const TmArgs* __restrict__ args, int inst, double* sm) { tm_body(args[inst], sm, 0); }

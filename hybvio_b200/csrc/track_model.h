@@ -44,4 +44,7 @@ struct TmArgs {
 #ifdef __CUDACC__
 #include <cuda_runtime.h>
 cudaError_t tm_launch(const TmArgs& a, cudaStream_t s);      // grid = a.ntracks CTAs of TM_NT threads
+// Group launch (hv_ekf_group_visual_tracks): CTA i runs track dArgs[i].trackOffset of dArgs[i], a block in device memory; hArgs is the
+// host copy of the same blocks (hArgs[0].pdl: the launch follows a kernel of the chains on the stream)
+cudaError_t tm_launch_group(const TmArgs* hArgs, const TmArgs* dArgs, int count, cudaStream_t s);
 #endif

@@ -340,7 +340,8 @@ int hv_ekf_run_host(hv_ekf* ekf, const hv_ekf_op* ops, int nops, int* vu_status,
  * Refused before anything is issued, every filter untouched: HV_ERR_UNSUPPORTED for any other op (UNAUGMENT, a standalone SYMMETRIZE or
  * NORMALIZE, a measurement or augmentation that does not fit); HV_ERR_INVALID for NULL arrays, a NULL filter, list or measurement
  * pointer, count outside 1..HV_EKF_GROUP_MAX, filters of different contexts or state dimensions, a filter that appears twice, a bad
- * mode or shape, an unknown op kind or a discarded-pose index out of range. The caller falls back to per-filter calls. */
+ * mode or shape, an unknown op kind or a discarded-pose index out of range. The caller falls back to per-filter calls.
+ * The visual-update chains of a group (hv_ekf_visual_tracks) have their own group call, hv_ekf_group_visual_tracks, below. */
 #define HV_EKF_GROUP_MAX 64
 int hv_ekf_group_run_device(hv_ekf* const* ekfs, int count, const hv_ekf_op* const* ops, const int* nops);
 
@@ -432,6 +433,28 @@ typedef struct hv_track_result {
 } hv_track_result;
 int hv_ekf_visual_tracks(hv_ekf* ekf, const hv_track_obs* tracks, int ntracks, const hv_visual_update_params* params,
                          hv_track_result* out, int* successful_updates);
+/* The visual-update chains of many independent filters of ONE context (several sessions per process; the counterpart of
+ * hv_ekf_group_run_device): for every i, the effect of hv_ekf_visual_tracks(ekfs[i], tracks[i], ntracks[i], &params[i], out[i],
+ * &successful_updates[i]) -- m, P, the pose count, the hv_track_result records and the successful-update count are bit-identical,
+ * lookahead included -- with the launches of one chain: step k is track k of every filter that still has tracks to issue, as one
+ * launch of the model kernel (a CTA per filter), one of the cluster kernel (a cluster per filter: check + update) and, in a step where
+ * a filter uses the separate form (chi_outlier_r < 0 or visual_r <= 0), one more for the updates of those filters. A group costs the
+ * launches of its longest chain. The host synchronises once per `lookahead` steps for all filters together (with different lookaheads:
+ * whenever a filter reaches the end of one of its windows); a filter with max_successful_updates reached at a synchronisation is not
+ * issued further, and its later tracks get the records of tracks the per-filter call never issues. Synchronises before it returns;
+ * HV_EKF_NO_PDL keeps its meaning. Work queued for a filter by earlier calls is issued first.
+ * Per filter: ntracks[i] (0: the filter is left untouched, its count is 0; tracks[i] and out[i] may then be NULL), params[i] and the
+ * camera model (mono or stereo) may differ. successful_updates: count entries, or NULL.
+ * Refused before anything is issued, every filter untouched: HV_ERR_INVALID for NULL arrays, a NULL filter, a NULL tracks[i] / out[i]
+ * where ntracks[i] > 0, a negative ntracks[i], count outside 1..HV_EKF_GROUP_MAX, filters of different contexts or state dimensions, a
+ * filter that appears twice, a malformed track (as hv_ekf_track_models checks them); HV_ERR_STATE for a filter without
+ * hv_ekf_set_camera_model; HV_ERR_UNSUPPORTED for a track whose measurement does not fit the cluster kernel whole (the group has no
+ * row-chunked form: every track of up to 84 rows fits at N = 160 and at N = 62); the message names the filter and the track, and the
+ * caller falls back to per-filter calls. An innovation covariance that is not positive definite in any filter returns HV_ERR_STATE after
+ * every result has been written, as the per-filter call does; the message names the (first such) filter. A single filter is faster
+ * through hv_ekf_visual_tracks (DESIGN.md 4.5b). */
+int hv_ekf_group_visual_tracks(hv_ekf* const* ekfs, int count, const hv_track_obs* const* tracks, const int* ntracks,
+                               const hv_visual_update_params* params, hv_track_result* const* out, int* successful_updates);
 /* Test / debug: copies H (rows x cols), f (rows) and d pf / d (poses, t) (3 x (7 npose + 1), column-major, after the stereo
  * sum) of track `track` of the last hv_ekf_track_models call to the host; any pointer may be NULL. */
 int hv_ekf_track_model_download(hv_ekf* ekf, int track, double* H, double* f, double* dpf);
