@@ -76,6 +76,19 @@ class LkJob(ctypes.Structure):
                 ("d_status", c_void_p), ("d_track_status", c_void_p), ("n", c_int), ("use_initial", c_int)]
 
 
+class CornerJob(ctypes.Structure):
+    """hv_corner_job: one session's list in the batched detect / select calls"""
+    _fields_ = [("pyr", c_void_p), ("d_kp", c_void_p), ("nkp", c_int), ("d_prev_xy", c_void_p), ("nprev", c_int),
+                ("mask_radius", c_int), ("max_tracks", c_int), ("d_corners", c_void_p), ("capacity", c_int), ("d_count", c_void_p)]
+
+
+class SubpixJob(ctypes.Structure):
+    """hv_subpix_job: one session's points in the batched sub-pixel refinement"""
+    _fields_ = [("pyr", c_void_p), ("d_xy", c_void_p), ("n", c_int)]
+
+
+CORNER_BATCH_MAX = 64   # HV_CORNER_BATCH_MAX
+
 _lib = None
 
 
@@ -120,6 +133,9 @@ def load():
     lib.hv_gftt_corners.argtypes = [c_void_p, c_void_p, c_int, c_int, ctypes.c_float, c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p]
     lib.hv_subpix_refine.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_double]
     lib.hv_subpix_refine_device.argtypes = lib.hv_subpix_refine.argtypes
+    lib.hv_gftt_detect_batch_device.argtypes = [c_void_p, ctypes.POINTER(CornerJob), c_int, c_int, c_int, ctypes.c_float]
+    lib.hv_gftt_select_batch_device.argtypes = [c_void_p, ctypes.POINTER(CornerJob), c_int]
+    lib.hv_subpix_refine_batch_device.argtypes = [c_void_p, ctypes.POINTER(SubpixJob), c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_double]
     _bind_ekf(lib)
     _lib = lib
     return lib
@@ -312,6 +328,23 @@ class Context:
         check(self.lib.hv_gftt_select_device(self.h, _ptr(d_kp), d_kp.numel() // 3, _ptr(d_prev), nprev, mask_radius, max_tracks,
                                              _ptr(d_corners), d_corners.numel() // 2, _ptr(d_count)), "hv_gftt_select_device")
 
+    # ---- the new-corner step of many sessions: one launch per call (see corner_job / subpix_job for the jobs)
+    def gftt_detect_batch_device(self, jobs, block_size=3, cell=32, min_response=1e-3):
+        """hv_gftt_detect_batch_device: every job's key points (d_kp) from level 0 of its pyramid; asynchronous."""
+        J = (CornerJob * len(jobs))(*jobs)
+        check(self.lib.hv_gftt_detect_batch_device(self.h, J, len(jobs), block_size, cell, min_response), "hv_gftt_detect_batch_device")
+
+    def gftt_select_batch_device(self, jobs):
+        """hv_gftt_select_batch_device: every job's corner list and count from its nkp key points; asynchronous."""
+        J = (CornerJob * len(jobs))(*jobs)
+        check(self.lib.hv_gftt_select_batch_device(self.h, J, len(jobs)), "hv_gftt_select_batch_device")
+
+    def subpix_refine_batch_device(self, jobs, win=(5, 5), zero_zone=(-1, -1), criteria=(3, 30, 0.01)):
+        """hv_subpix_refine_batch_device: every job's points refined in place on level 0 of its pyramid; asynchronous."""
+        J = (SubpixJob * len(jobs))(*jobs)
+        check(self.lib.hv_subpix_refine_batch_device(self.h, J, len(jobs), win[0], win[1], zero_zone[0], zero_zone[1],
+                                                     criteria[0], criteria[1], criteria[2]), "hv_subpix_refine_batch_device")
+
     def lk_track_device(self, prev, nxt, d_prev, d_next, d_status, d_ts, n, use_initial, max_iter=20, eps=0.03, min_eig=1e-3):
         check(self.lib.hv_lk_track_device(self.h, prev.h, nxt.h, _ptr(d_prev), _ptr(d_next), _ptr(d_status), _ptr(d_ts), n,
                                           1 if use_initial else 0, max_iter, eps, min_eig), "hv_lk_track_device")
@@ -321,6 +354,31 @@ class Context:
         """The same launch on a stream of the caller; d_init (or None): predicted end points, read from their own buffer."""
         check(self.lib.hv_lk_track_device_on_stream(self.h, c_void_p(int(cuda_stream)), prev.h, nxt.h, _ptr(d_prev), _ptr(d_init), _ptr(d_next),
                                                     _ptr(d_status), _ptr(d_ts), n, max_iter, eps, min_eig), "hv_lk_track_device_on_stream")
+
+
+def _check_cuda_buffer(t):
+    assert t.is_cuda and t.is_contiguous() and t.element_size() == 4
+    return t
+
+
+def corner_job(pyr=None, d_kp=None, d_corners=None, d_count=None, d_prev=None, mask_radius=0, max_tracks=150, nkp=None):
+    """A CornerJob on contiguous CUDA tensors: d_kp (nkp, 3) float32 (nkp: all its rows unless given), d_corners (capacity, 2) float32,
+    d_count (1,) int32, d_prev (nprev, 2) float32 or None; pyr a Pyramid (detect) or None (select only). The tensors must outlive the
+    calls that use the job."""
+    for t in (d_kp, d_corners, d_count, d_prev):
+        if t is not None:
+            _check_cuda_buffer(t)
+    if nkp is None:
+        nkp = 0 if d_kp is None else d_kp.numel() // 3
+    return CornerJob(None if pyr is None else pyr.h.value, _ptr(d_kp), nkp,
+                     _ptr(d_prev), 0 if d_prev is None else d_prev.numel() // 2, mask_radius, max_tracks,
+                     _ptr(d_corners), 0 if d_corners is None else d_corners.numel() // 2, _ptr(d_count))
+
+
+def subpix_job(pyr, d_xy, n=None):
+    """A SubpixJob: the first n (all) points of a contiguous (m, 2) float32 CUDA tensor on level 0 of pyr."""
+    _check_cuda_buffer(d_xy)
+    return SubpixJob(pyr.h.value, _ptr(d_xy), d_xy.numel() // 2 if n is None else n)
 
 
 def gftt_select_capacity(nkp, mask_radius, max_tracks):

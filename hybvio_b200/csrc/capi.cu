@@ -1,6 +1,7 @@
 // hybvio_b200/csrc/capi.cu -- C ABI (include/hybvio_b200.h): context, image pyramid, Lucas-Kanade.
 // The EKF entry points live in ekf_capi.cu.
 #include "capi_internal.h"
+#include <climits>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -610,8 +611,8 @@ int hv_gftt_corners(hv_ctx* c, hv_pyr* pyr, int blockSize, int cell, float minRe
 }
 
 // ------------------------------------------------------------------------------------------------ sub-pixel refinement (cornerSubPix)
-static int subpix_args(const char* who, hv_ctx* c, hv_pyr* pyr, int n, int hw, int hh, int zw, int zh, int criteriaType, int maxCount,
-                       double epsilon, SubpixArgs& a)
+// the checks of one point list on pyr's level 0
+static int subpix_check(const char* who, hv_ctx* c, hv_pyr* pyr, int n, int hw, int hh)
 {
     if (!c || !pyr || pyr->ctx != c || n < 0) { hv_set_error("%s: invalid context / pyramid / count", who); return HV_ERR_INVALID; }
     if (hw < 1 || hh < 1 || hw > HV_SUBPIX_MAX_HALF || hh > HV_SUBPIX_MAX_HALF) {
@@ -623,6 +624,15 @@ static int subpix_args(const char* who, hv_ctx* c, hv_pyr* pyr, int n, int hw, i
         hv_set_error("%s: image %d x %d smaller than the window needs (%d x %d)", who, L.w, L.h, 2 * hw + 5, 2 * hh + 5);
         return HV_ERR_INVALID;
     }
+    return HV_OK;
+}
+
+static int subpix_args(const char* who, hv_ctx* c, hv_pyr* pyr, int n, int hw, int hh, int zw, int zh, int criteriaType, int maxCount,
+                       double epsilon, SubpixArgs& a)
+{
+    int rc = subpix_check(who, c, pyr, n, hw, hh);
+    if (rc != HV_OK) return rc;
+    const HvLevel& L = pyr->desc.lv[0];
     memset(&a, 0, sizeof(a));
     a.gray = L.gray; a.pitch = L.gpitch; a.w = L.w; a.h = L.h; a.n = n; a.hw = hw; a.hh = hh;
     // criteria and mask exactly as cv::cornerSubPix forms them (OpenCV's MIN / MAX macros; std::exp(float))
@@ -701,6 +711,103 @@ int hv_subpix_refine(hv_ctx* c, hv_pyr* pyr, float* xy, int n, int hw, int hh, i
         HV_CUDA(cudaStreamSynchronize(c->stream));
     }
     memcpy(xy, hs, bytes);
+    return HV_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ the corner step of many sessions (N2)
+// Each call checks every job with the checks of the per-session call and refuses before anything is launched; then one launch on the
+// context's stream does what the per-session calls would do for every job, bit for bit. The argument blocks travel as kernel parameters.
+static_assert(HV_CORNER_BATCH_MAX == 64, "batch size of the header and of the kernels");
+
+static int corner_batch_check(const char* who, hv_ctx* c, const void* jobs, int njobs)
+{
+    if (!c || !jobs) { hv_set_error("%s: NULL context or jobs", who); return HV_ERR_INVALID; }
+    if (njobs < 1 || njobs > HV_CORNER_BATCH_MAX) { hv_set_error("%s: %d jobs (1..%d per call)", who, njobs, HV_CORNER_BATCH_MAX); return HV_ERR_INVALID; }
+    return HV_OK;
+}
+
+int hv_gftt_detect_batch_device(hv_ctx* c, const hv_corner_job* jobs, int njobs, int blockSize, int cell, float minResponse)
+{
+    int rc = corner_batch_check("hv_gftt_detect_batch_device", c, jobs, njobs);
+    if (rc != HV_OK) return rc;
+    GfttBatchArgs b;
+    memset(&b, 0, sizeof(b));
+    int ctas = 0;
+    for (int j = 0; j < njobs; j++) {
+        char who[64];
+        snprintf(who, sizeof(who), "hv_gftt_detect_batch_device job %d", j);
+        rc = gftt_args(who, c, jobs[j].pyr, blockSize, cell, minResponse, b.job[j]);
+        if (rc != HV_OK) return rc;
+        if (!jobs[j].d_kp) { hv_set_error("%s: NULL key points", who); return HV_ERR_INVALID; }
+        b.job[j].kp = jobs[j].d_kp;
+        const int cx = b.job[j].w / cell, cy = b.job[j].h / cell;       // as hv_launch_gftt: an image smaller than a cell adds no CTA
+        b.first[j] = ctas;
+        b.cellsX[j] = cx;
+        if (cx > 0 && cy > 0) ctas += cx * cy;                          // at most 64 x (32767 / 2)^2: no overflow
+    }
+    for (int j = njobs; j <= HV_CORNER_BATCH_MAX; j++) b.first[j] = ctas;
+    if (ctas == 0) return HV_OK;
+    HV_CUDA(cudaSetDevice(c->device));
+    HV_CUDA(hv_launch_gftt_batch(b, njobs, c->stream));
+    c->launches += 1;
+    return HV_OK;
+}
+
+int hv_gftt_select_batch_device(hv_ctx* c, const hv_corner_job* jobs, int njobs)
+{
+    int rc = corner_batch_check("hv_gftt_select_batch_device", c, jobs, njobs);
+    if (rc != HV_OK) return rc;
+    GfttSelectBatchArgs b;
+    memset(&b, 0, sizeof(b));
+    int maxPow2 = 2;
+    for (int j = 0; j < njobs; j++) {
+        const hv_corner_job& J = jobs[j];
+        char who[64];
+        snprintf(who, sizeof(who), "hv_gftt_select_batch_device job %d", j);
+        if (!J.d_corners || !J.d_count || (J.nkp > 0 && !J.d_kp) || (J.nprev > 0 && !J.d_prev_xy)) {
+            hv_set_error("%s: NULL buffer", who);
+            return HV_ERR_INVALID;
+        }
+        GfttSelectArgs& a = b.job[j];
+        int need = 0;
+        rc = select_args(who, J.nkp, J.nprev, J.mask_radius, J.max_tracks, J.capacity, a, &need);
+        if (rc != HV_OK) return rc;
+        a.kp = J.d_kp; a.prev = J.d_prev_xy; a.out = J.d_corners; a.count = J.d_count;
+        if (a.pow2 > maxPow2) maxPow2 = a.pow2;
+    }
+    HV_CUDA(cudaSetDevice(c->device));
+    HV_CUDA(hv_launch_gftt_select_batch(b, njobs, maxPow2, c->stream));   // a job with nkp = 0 writes count 0 and its padding only
+    c->launches += 1;
+    return HV_OK;
+}
+
+int hv_subpix_refine_batch_device(hv_ctx* c, const hv_subpix_job* jobs, int njobs, int hw, int hh, int zw, int zh, int criteriaType,
+                                  int maxCount, double epsilon)
+{
+    int rc = corner_batch_check("hv_subpix_refine_batch_device", c, jobs, njobs);
+    if (rc != HV_OK) return rc;
+    SubpixBatchArgs b;
+    memset(&b, 0, sizeof(b));
+    long long points = 0;
+    for (int j = 0; j < njobs; j++) {
+        const hv_subpix_job& J = jobs[j];
+        char who[64];
+        snprintf(who, sizeof(who), "hv_subpix_refine_batch_device job %d", j);
+        // the window, criteria and mask are the batch's: formed once, with the checks of job 0
+        rc = j == 0 ? subpix_args(who, c, J.pyr, J.n, hw, hh, zw, zh, criteriaType, maxCount, epsilon, b.s) : subpix_check(who, c, J.pyr, J.n, hw, hh);
+        if (rc != HV_OK) return rc;
+        if (J.n > 0 && !J.d_xy) { hv_set_error("%s: NULL points", who); return HV_ERR_INVALID; }
+        const HvLevel& L = J.pyr->desc.lv[0];
+        b.job[j] = SubpixJob{L.gray, L.gpitch, L.w, L.h, (float2*)J.d_xy, J.n};
+        b.first[j] = (int)points;
+        points += J.n;
+        if (points > INT_MAX) { hv_set_error("%s: more than %d points in one batch", who, INT_MAX); return HV_ERR_INVALID; }
+    }
+    for (int j = njobs; j <= HV_CORNER_BATCH_MAX; j++) b.first[j] = (int)points;
+    if (points == 0) return HV_OK;
+    HV_CUDA(cudaSetDevice(c->device));
+    HV_CUDA(hv_launch_subpix_batch(b, njobs, c->stream));
+    c->launches += 1;
     return HV_OK;
 }
 

@@ -17,19 +17,23 @@
 // operation an explicitly rounded intrinsic (no FMA contraction): the response is bit-identical to oracle/hv_oracle_gftt.c, which
 // differs from the compiled reference only by the order of the box sum (running sums in OpenCV; <= 1e-9 absolute, tests/test_oracle_gftt.py).
 // HBM traffic: the image is read once (each pixel by at most 4 cells through L2): w * h bytes in, 12 bytes per cell out.
+//
+// hv_gftt_batch_kernel runs the same cell body for the cells of up to HV_CORNER_BATCH_MAX images (one per session) in one flattened grid:
+// CTA b belongs to the job j with first[j] <= b < first[j + 1] (a prefix sum of the cell counts, formed on the host; hv_batch_job).
 #include "hv_common.cuh"
 
 #define GFTT_NT 256
 #define GFTT_MAX_CELL 32
 
-__global__ void __launch_bounds__(GFTT_NT) hv_gftt_kernel(GfttArgs a)
+// the key point of cell (cellX, cellY) of a grid cellsX cells wide, by one CTA of GFTT_NT threads
+__device__ __forceinline__ void hv_gftt_cell(const GfttArgs& a, int cellX, int cellY, int cellsX)
 {
     constexpr int R = GFTT_MAX_CELL + 4, C = GFTT_MAX_CELL + 2;
     __shared__ float g[R][R + 1];
     __shared__ float cxx[C][C + 1], cxy[C][C + 1], cyy[C][C + 1];
     __shared__ float s_val[GFTT_NT / 32];
     __shared__ int s_idx[GFTT_NT / 32];
-    const int bs = a.cell, x0 = blockIdx.x * bs, y0 = blockIdx.y * bs, tid = threadIdx.x;
+    const int bs = a.cell, x0 = cellX * bs, y0 = cellY * bs, tid = threadIdx.x;
     const int rw = bs + 4, cw = bs + 2;
     // ---- gray region [x0 - 2, x0 + bs + 2) x [y0 - 2, y0 + bs + 2), reflected into the image
     for (int i = tid; i < rw * rw; i += GFTT_NT) {
@@ -83,7 +87,7 @@ __global__ void __launch_bounds__(GFTT_NT) hv_gftt_kernel(GfttArgs a)
     if (tid == 0) {
         for (int q = 1; q < GFTT_NT / 32; q++)
             if (s_val[q] > best || (s_val[q] == best && s_idx[q] < bidx)) { best = s_val[q]; bidx = s_idx[q]; }
-        float* out = a.kp + 3 * ((size_t)blockIdx.y * gridDim.x + blockIdx.x);
+        float* out = a.kp + 3 * ((size_t)cellY * cellsX + cellX);
         const bool found = best > -1e10f;
         out[0] = found ? (float)(x0 + bidx % bs) : 0.0f;               // the reference leaves (0, 0) when no pixel of the cell qualifies
         out[1] = found ? (float)(y0 + bidx / bs) : 0.0f;
@@ -96,10 +100,30 @@ __global__ void __launch_bounds__(GFTT_NT) hv_gftt_kernel(GfttArgs a)
     }
 }
 
+__global__ void __launch_bounds__(GFTT_NT) hv_gftt_kernel(GfttArgs a)
+{
+    hv_gftt_cell(a, blockIdx.x, blockIdx.y, gridDim.x);
+}
+
+__global__ void __launch_bounds__(GFTT_NT) hv_gftt_batch_kernel(const __grid_constant__ GfttBatchArgs b)
+{
+    const int cta = blockIdx.x, j = hv_batch_job(b.first, cta);
+    const int k = cta - b.first[j], cellsX = b.cellsX[j];
+    hv_gftt_cell(b.job[j], k % cellsX, k / cellsX, cellsX);
+}
+
 cudaError_t hv_launch_gftt(const GfttArgs& a, cudaStream_t stream)
 {
     const int cx = a.w / a.cell, cy = a.h / a.cell;                    // integer division, as the reference (feature_detector.cpp:395-396)
     if (cx <= 0 || cy <= 0) return cudaSuccess;
     hv_gftt_kernel<<<dim3(cx, cy), GFTT_NT, 0, stream>>>(a);
+    return cudaGetLastError();
+}
+
+cudaError_t hv_launch_gftt_batch(const GfttBatchArgs& b, int njobs, cudaStream_t stream)
+{
+    const int ctas = b.first[njobs];
+    if (ctas <= 0) return cudaSuccess;
+    hv_gftt_batch_kernel<<<ctas, GFTT_NT, 0, stream>>>(b);
     return cudaGetLastError();
 }

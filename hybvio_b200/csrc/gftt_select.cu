@@ -18,6 +18,8 @@
 //  * Distance test as the reference writes it, (c.x - p.x)^2 + (c.y - p.y)^2 < (float)(r * r) with c the other point, in fp32 with every
 //    operation an explicitly rounded intrinsic (no FMA contraction).
 // NaN responses (which the detector never produces) are outside the contract: the reference's insertion order around them is not a sort.
+//
+// hv_gftt_select_batch_kernel runs the same list body for up to HV_CORNER_BATCH_MAX lists (one per session): CTA j is list j.
 #include "hv_common.cuh"
 
 #define SEL_NT 1024
@@ -37,7 +39,8 @@ __device__ __forceinline__ bool hv_select_near(float ox, float oy, float cx, flo
     return __fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)) < r2;
 }
 
-__global__ void __launch_bounds__(SEL_NT) hv_gftt_select_kernel(const __grid_constant__ GfttSelectArgs a)
+// list a, by one CTA of SEL_NT threads
+__device__ __forceinline__ void hv_gftt_select_list(const GfttSelectArgs& a)
 {
     extern __shared__ __align__(16) unsigned char select_smem[];
     unsigned long long* key = (unsigned long long*)select_smem;       // pow2 sort keys; afterwards slot k holds sorted point k ...
@@ -117,9 +120,20 @@ __global__ void __launch_bounds__(SEL_NT) hv_gftt_select_kernel(const __grid_con
     }
 }
 
+__global__ void __launch_bounds__(SEL_NT) hv_gftt_select_kernel(const __grid_constant__ GfttSelectArgs a)
+{
+    hv_gftt_select_list(a);
+}
+
+// one list per CTA; each CTA sorts its own pow2 keys in the dynamic shared memory sized for the largest
+__global__ void __launch_bounds__(SEL_NT) hv_gftt_select_batch_kernel(const __grid_constant__ GfttSelectBatchArgs b)
+{
+    hv_gftt_select_list(b.job[blockIdx.x]);
+}
+
 #include "hv_device_once.cuh"
 
-static bool g_select_attr_set[64];
+static bool g_select_attr_set[64], g_select_batch_attr_set[64];
 
 cudaError_t hv_launch_gftt_select(const GfttSelectArgs& a, cudaStream_t stream)
 {
@@ -129,5 +143,16 @@ cudaError_t hv_launch_gftt_select(const GfttSelectArgs& a, cudaStream_t stream)
         if (e != cudaSuccess) return e;
     }
     hv_gftt_select_kernel<<<1, SEL_NT, (size_t)a.pow2 * sizeof(unsigned long long), stream>>>(a);
+    return cudaGetLastError();
+}
+
+cudaError_t hv_launch_gftt_select_batch(const GfttSelectBatchArgs& b, int njobs, int maxPow2, cudaStream_t stream)
+{
+    if (hv_first_use_on_device(g_select_batch_attr_set)) {
+        cudaError_t e = cudaFuncSetAttribute(hv_gftt_select_batch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             (int)(HV_GFTT_SELECT_MAX_KP * sizeof(unsigned long long)));
+        if (e != cudaSuccess) return e;
+    }
+    hv_gftt_select_batch_kernel<<<njobs, SEL_NT, (size_t)maxPow2 * sizeof(unsigned long long), stream>>>(b);
     return cudaGetLastError();
 }

@@ -85,6 +85,29 @@ struct GfttArgs {
 
 cudaError_t hv_launch_gftt(const GfttArgs& a, cudaStream_t stream);
 
+// Batches of the corner step (detect, select, refine): one job per session, at most HV_CORNER_BATCH_MAX per launch. Every argument
+// block travels as a __grid_constant__ kernel parameter (at most 32764 bytes on sm_90).
+#define HV_CORNER_BATCH_MAX 64
+#define HV_KERNEL_PARAM_MAX 32764
+
+// The job of CTA b in a flattened grid: the last j with first[j] <= b, where first[] is the prefix sum of the jobs' CTA counts (a job
+// without CTAs repeats its successor's start) padded with the grid size up to HV_CORNER_BATCH_MAX. Six steps whatever the batch size.
+__host__ __device__ __forceinline__ int hv_batch_job(const int* first, int b)
+{
+    int j = 0;
+#pragma unroll
+    for (int step = HV_CORNER_BATCH_MAX / 2; step > 0; step >>= 1)
+        if (first[j + step] <= b) j += step;
+    return j;
+}
+struct GfttBatchArgs {
+    GfttArgs job[HV_CORNER_BATCH_MAX];        // hostFlag NULL
+    int first[HV_CORNER_BATCH_MAX + 1];       // first CTA (cell) of job j in the flattened grid; first[njobs ..] = the grid
+    int cellsX[HV_CORNER_BATCH_MAX];
+};
+static_assert(sizeof(GfttBatchArgs) <= HV_KERNEL_PARAM_MAX, "detect batch arguments exceed the kernel-parameter space");
+cudaError_t hv_launch_gftt_batch(const GfttBatchArgs& b, int njobs, cudaStream_t stream);
+
 // ---- corner selection launch description (gftt_select.cu): the detector's sort, resize quirk and applyMinDistance
 #define HV_GFTT_SELECT_MAX_KP 16384   // key points per call: one CTA, the sort keys in opt-in shared memory (128 KB)
 #define HV_GFTT_SELECT_MAX_RADIUS 46340   // mask_radius^2 still fits the reference's int product
@@ -102,6 +125,13 @@ struct GfttSelectArgs {
 
 cudaError_t hv_launch_gftt_select(const GfttSelectArgs& a, cudaStream_t stream);
 
+struct GfttSelectBatchArgs {
+    GfttSelectArgs job[HV_CORNER_BATCH_MAX];  // CTA j is list j; hostFlag NULL
+};
+static_assert(sizeof(GfttSelectBatchArgs) <= HV_KERNEL_PARAM_MAX, "select batch arguments exceed the kernel-parameter space");
+// maxPow2: the largest job[j].pow2, which sizes the dynamic shared memory of every CTA
+cudaError_t hv_launch_gftt_select_batch(const GfttSelectBatchArgs& b, int njobs, int maxPow2, cudaStream_t stream);
+
 // ---- sub-pixel corner refinement launch description (subpix.cu)
 #define HV_SUBPIX_MAX_HALF 15        // half-window per axis: a 31 x 31 window at most
 struct SubpixArgs {
@@ -115,6 +145,15 @@ struct SubpixArgs {
 };
 
 cudaError_t hv_launch_subpix(const SubpixArgs& a, cudaStream_t stream);
+
+struct SubpixJob { const uint8_t* gray; int pitch, w, h; float2* xy; int n; };
+struct SubpixBatchArgs {
+    SubpixArgs s;                             // window, criteria and mask of the whole batch (gray, xy, n and the flag unused)
+    SubpixJob job[HV_CORNER_BATCH_MAX];
+    int first[HV_CORNER_BATCH_MAX + 1];       // first CTA (point) of job j in the flattened grid; first[njobs ..] = the grid
+};
+static_assert(sizeof(SubpixBatchArgs) <= HV_KERNEL_PARAM_MAX, "sub-pixel batch arguments exceed the kernel-parameter space");
+cudaError_t hv_launch_subpix_batch(const SubpixBatchArgs& b, int njobs, cudaStream_t stream);
 
 // ---- frame ingest (ingest.cu)
 #define HV_REMAP_INVALID (-32768)

@@ -8,6 +8,10 @@
 // Every float and double operation is an explicitly rounded intrinsic (no FMA contraction) with OpenCV's casts: the result is
 // bit-identical to oracle/hv_oracle_subpix.c, and with it to cv::cornerSubPix built without IPP. The mask (exp on the host) arrives
 // with the arguments.
+//
+// hv_subpix_batch_kernel runs the same corner body for the points of up to HV_CORNER_BATCH_MAX lists (one per session, each on its own
+// image) in one flattened grid: CTA g refines point g - first[j] of the job j with first[j] <= g < first[j + 1]. The window, criteria and
+// mask are the batch's.
 #include "hv_common.cuh"
 #include <cfloat>
 
@@ -20,11 +24,11 @@ __host__ __device__ inline size_t hv_subpix_smem_bytes(int hw, int hh)
 }
 
 // cv::getRectSubPix(gray, Size(pw, ph), Point2f(cx, cy), patch, CV_32F), one element per lane and step
-__device__ void hv_subpix_patch(const SubpixArgs& a, int pw, int ph, float cx, float cy, float* patch, int lane)
+__device__ void hv_subpix_patch(const uint8_t* gray, int pitch, int w, int h, int pw, int ph, float cx, float cy, float* patch, int lane)
 {
     const float x = __fsub_rn(cx, (float)(pw - 1) * 0.5f), y = __fsub_rn(cy, (float)(ph - 1) * 0.5f);
     const int ipx = __float2int_rd(x), ipy = __float2int_rd(y);
-    if (0 <= ipx && ipx + pw < a.w && 0 <= ipy && ipy + ph < a.h) {
+    if (0 <= ipx && ipx + pw < w && 0 <= ipy && ipy + ph < h) {
         // getRectSubPix_8u32f: the rectangle lies inside the image. Its running `prev` is the previous column's t scaled by s, so every
         // element can be formed on its own.
         float fa = __fsub_rn(x, (float)ipx);
@@ -34,8 +38,8 @@ __device__ void hv_subpix_patch(const SubpixArgs& a, int pw, int ph, float cx, f
         const double s = hv_dsub(1.0, (double)fa) / (double)fa;
         for (int e = lane; e < pw * ph; e += 32) {
             const int i = e / pw, j = e - i * pw;
-            const uint8_t* r0 = a.gray + (size_t)(ipy + i) * a.pitch + ipx;
-            const uint8_t* r1 = r0 + a.pitch;
+            const uint8_t* r0 = gray + (size_t)(ipy + i) * pitch + ipx;
+            const uint8_t* r1 = r0 + pitch;
             const float t = __fadd_rn(__fmul_rn(a12, (float)__ldg(r0 + j + 1)), __fmul_rn(a22, (float)__ldg(r1 + j + 1)));
             float prev;
             if (j == 0) {
@@ -53,17 +57,17 @@ __device__ void hv_subpix_patch(const SubpixArgs& a, int pw, int ph, float cx, f
     const float fa = __fsub_rn(x, (float)ipx), fb = __fsub_rn(y, (float)ipy), ia = __fsub_rn(1.f, fa), ib = __fsub_rn(1.f, fb);
     const float a11 = __fmul_rn(ia, ib), a12 = __fmul_rn(fa, ib), a21 = __fmul_rn(ia, fb), a22 = __fmul_rn(fa, fb), b1 = ib, b2 = fb;
     int col0 = ipx >= 0 ? ipx : 0, rx = ipx >= 0 ? 0 : (-ipx > pw ? pw : -ipx), rw;
-    if (ipx < a.w - pw) rw = pw;
-    else { rw = a.w - ipx - 1; if (rw < 0) { col0 += rw; rw = 0; } }
+    if (ipx < w - pw) rw = pw;
+    else { rw = w - ipx - 1; if (rw < 0) { col0 += rw; rw = 0; } }
     int row0 = ipy >= 0 ? ipy : 0, ry = ipy >= 0 ? 0 : -ipy, rh;
-    if (ipy < a.h - ph) rh = ph;
-    else { rh = a.h - ipy - 1; if (rh < 0) { row0 += rh; rh = 0; } }
+    if (ipy < h - ph) rh = ph;
+    else { rh = h - ipy - 1; if (rh < 0) { row0 += rh; rh = 0; } }
     for (int e = lane; e < pw * ph; e += 32) {
         const int i = e / pw, j = e - i * pw;
         // the source row advances after every patch row i with ry <= i < rh
         const int adv = (i < rh ? i : rh) - ry, row = row0 + (adv > 0 ? adv : 0), row2 = (i < ry || i >= rh) ? row : row + 1;
-        const uint8_t* s1 = a.gray + (size_t)row * a.pitch + (col0 - rx);
-        const uint8_t* s2 = a.gray + (size_t)row2 * a.pitch + (col0 - rx);
+        const uint8_t* s1 = gray + (size_t)row * pitch + (col0 - rx);
+        const uint8_t* s2 = gray + (size_t)row2 * pitch + (col0 - rx);
         float v;
         if (j >= rw) v = __fadd_rn(__fmul_rn((float)__ldg(s1 + rw), b1), __fmul_rn((float)__ldg(s2 + rw), b2));
         else if (j < rx) v = __fadd_rn(__fmul_rn((float)__ldg(s1 + rx), b1), __fmul_rn((float)__ldg(s2 + rx), b2));
@@ -73,7 +77,8 @@ __device__ void hv_subpix_patch(const SubpixArgs& a, int pw, int ph, float cx, f
     }
 }
 
-__global__ void __launch_bounds__(32) hv_subpix_kernel(const __grid_constant__ SubpixArgs a)
+// the refined position of the corner *xy of the image (gray, pitch, w, h), with the window, criteria and mask of a, by one warp
+__device__ __forceinline__ float2 hv_subpix_corner(const SubpixArgs& a, const uint8_t* gray, int pitch, int w, int h, const float2* xy)
 {
     extern __shared__ __align__(16) unsigned char subpix_smem[];
     const int lane = threadIdx.x, hw = a.hw, hh = a.hh;
@@ -82,13 +87,13 @@ __global__ void __launch_bounds__(32) hv_subpix_kernel(const __grid_constant__ S
     float* patch = (float*)(term + 5 * taps);             // ph x pw
     float* mask = patch + pw * ph;                        // wh x ww
     for (int k = lane; k < taps; k += 32) mask[k] = a.mask[k];
-    const float2 cT = a.xy[blockIdx.x];
+    const float2 cT = *xy;
     float cx = cT.x, cy = cT.y;
     // cv::cornerSubPix asserts a start inside the image (the host entry point checks it); the device entry point leaves such a point as it is
-    if (cx >= 0.f && cx < (float)a.w && cy >= 0.f && cy < (float)a.h) {
+    if (cx >= 0.f && cx < (float)w && cy >= 0.f && cy < (float)h) {
         for (int iter = 0;;) {
             __syncwarp();
-            hv_subpix_patch(a, pw, ph, cx, cy, patch, lane);
+            hv_subpix_patch(gray, pitch, w, h, pw, ph, cx, cy, patch, lane);
             __syncwarp();
             for (int k = lane; k < taps; k += 32) {
                 const int i = k / ww, j = k - i * ww;
@@ -116,15 +121,21 @@ __global__ void __launch_bounds__(32) hv_subpix_kernel(const __grid_constant__ S
             const float ny = (float)__dadd_rn(hv_dsub((double)cy, __dmul_rn(__dmul_rn(B, scale), bb1)), __dmul_rn(__dmul_rn(A, scale), bb2));
             const float dx = __fsub_rn(nx, cx), dy = __fsub_rn(ny, cy);
             const float err = __fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy));            // float, as OpenCV's Point2f arithmetic
-            if (nx < 0.f || nx >= (float)a.w || ny < 0.f || ny >= (float)a.h) break;        // a step out of the image is not taken
+            if (nx < 0.f || nx >= (float)w || ny < 0.f || ny >= (float)h) break;        // a step out of the image is not taken
             cx = nx; cy = ny;
             if (!(++iter < a.maxIters && (double)err > a.eps2)) break;
         }
         // moved more than the window: poor convergence, the start point stands
         if (fabsf(__fsub_rn(cx, cT.x)) > (float)hw || fabsf(__fsub_rn(cy, cT.y)) > (float)hh) { cx = cT.x; cy = cT.y; }
     }
-    if (lane == 0) {
-        a.xy[blockIdx.x] = make_float2(cx, cy);
+    return make_float2(cx, cy);
+}
+
+__global__ void __launch_bounds__(32) hv_subpix_kernel(const __grid_constant__ SubpixArgs a)
+{
+    const float2 r = hv_subpix_corner(a, a.gray, a.pitch, a.w, a.h, a.xy + blockIdx.x);
+    if (threadIdx.x == 0) {
+        a.xy[blockIdx.x] = r;
         if (a.hostFlag) {
             __threadfence_system();
             const unsigned old = atomicAdd(a.doneCounter, 1u);
@@ -133,9 +144,26 @@ __global__ void __launch_bounds__(32) hv_subpix_kernel(const __grid_constant__ S
     }
 }
 
+__global__ void __launch_bounds__(32) hv_subpix_batch_kernel(const __grid_constant__ SubpixBatchArgs b)
+{
+    const int g = blockIdx.x, j = hv_batch_job(b.first, g);
+    const SubpixJob& J = b.job[j];
+    float2* xy = J.xy + (g - b.first[j]);
+    const float2 r = hv_subpix_corner(b.s, J.gray, J.pitch, J.w, J.h, xy);
+    if (threadIdx.x == 0) *xy = r;
+}
+
 cudaError_t hv_launch_subpix(const SubpixArgs& a, cudaStream_t stream)
 {
     if (a.n <= 0) return cudaSuccess;
     hv_subpix_kernel<<<a.n, 32, hv_subpix_smem_bytes(a.hw, a.hh), stream>>>(a);
+    return cudaGetLastError();
+}
+
+cudaError_t hv_launch_subpix_batch(const SubpixBatchArgs& b, int njobs, cudaStream_t stream)
+{
+    const int ctas = b.first[njobs];
+    if (ctas <= 0) return cudaSuccess;
+    hv_subpix_batch_kernel<<<ctas, 32, hv_subpix_smem_bytes(b.s.hw, b.s.hh), stream>>>(b);
     return cudaGetLastError();
 }

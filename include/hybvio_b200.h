@@ -172,6 +172,40 @@ int hv_subpix_refine(hv_ctx* ctx, hv_pyr* pyr, float* xy, int n, int win_w, int 
 int hv_subpix_refine_device(hv_ctx* ctx, hv_pyr* pyr, float* d_xy, int n, int win_w, int win_h, int zero_w, int zero_h,
                             int criteria_type, int max_count, double epsilon);   /* device xy, asynchronous */
 
+/* ---------------------------------------------------------------- the new-corner step of many sessions -------- */
+/* hv_gftt_detect_device, hv_gftt_select_device and hv_subpix_refine_device for up to HV_CORNER_BATCH_MAX independent lists (one per
+ * session sharing the context) in ONE launch each: every job's outputs are bit-identical to the per-session call's. Device buffers,
+ * asynchronous, on the context's stream; composes as
+ *   hv_gftt_detect_batch_device -> hv_gftt_select_batch_device -> hv_subpix_refine_batch_device -> hv_lk_track_batch_device
+ * (the stereo LK over every job's d_corners and capacity: one launch per 8 jobs). The parameters that shape a launch
+ * (block size, cell, response threshold; the sub-pixel window, zero zone and criteria) are the batch's; the rest is per job.
+ *   pyr          detect / refine: level 0 is the frame; pyramids may differ in size and pitch (select does not read it)
+ *   d_kp, nkp    (x, y, response) per cell: detect writes hv_gftt_cells' cells_x * cells_y of them (nkp unused), select reads nkp
+ *   d_prev_xy, nprev, mask_radius, max_tracks, d_corners, capacity, d_count: as hv_gftt_select_device (d_corners padded with
+ *                HV_CORNER_NONE up to capacity)
+ * Errors, for every job and before anything is launched: HV_ERR_INVALID for njobs outside 1..HV_CORNER_BATCH_MAX, a NULL context / jobs /
+ * pyramid / buffer (d_kp, d_prev_xy, d_xy may be NULL when their count is 0; select's d_kp is never written), a pyramid of another
+ * context, a negative count, max_tracks < 1, a capacity below the worst case, an image smaller than the sub-pixel window needs, or more
+ * than 2^31 - 1 points in a refine batch; HV_ERR_UNSUPPORTED for what the per-session calls refuse as such (block size other than 3, cell
+ * outside 2..32, more than 16384 key points in a job, a mask_radius above 46340, a half-window outside 1..15).
+ * Each call is one launch (ctx's launch count + 1); a detect batch in which no image holds a cell and a refine batch without points
+ * launch nothing. One session alone is served as well by the per-session calls (DESIGN.md 4.6 has the measured times). */
+#define HV_CORNER_BATCH_MAX 64
+typedef struct hv_corner_job {
+    hv_pyr* pyr;
+    float* d_kp; int nkp;
+    const float* d_prev_xy; int nprev;
+    int mask_radius, max_tracks;
+    float* d_corners; int capacity;
+    int* d_count;
+} hv_corner_job;
+int hv_gftt_detect_batch_device(hv_ctx* ctx, const hv_corner_job* jobs, int njobs, int block_size, int cell, float min_response);
+int hv_gftt_select_batch_device(hv_ctx* ctx, const hv_corner_job* jobs, int njobs);
+/* d_xy: n x (x, y) float32 on level 0 of pyr, refined in place (a point outside the image stays as it is, HV_CORNER_NONE padding too) */
+typedef struct hv_subpix_job { hv_pyr* pyr; float* d_xy; int n; } hv_subpix_job;
+int hv_subpix_refine_batch_device(hv_ctx* ctx, const hv_subpix_job* jobs, int njobs, int win_w, int win_h, int zero_w, int zero_h,
+                                  int criteria_type, int max_count, double epsilon);
+
 /* ---------------------------------------------------------------- frame ingest (SURVEY.md 8(f) N4) -------- */
 /* Device part of tracker::Image::Factory::build / buildStereo (src/tracker/image.cpp:243-308): colour -> gray
  * (accelerated-arrays pixelwiseAffine, image.cpp:360-366) and undistortion / rectification (UndistorterImplementation::undistort,
