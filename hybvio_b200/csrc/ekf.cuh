@@ -119,16 +119,18 @@ __device__ __forceinline__ void ekf_report(const EkfUpdateArgs& a, double st, do
     }
 }
 
-// Independent outlier checks against the same (m, P): one launch, one 8-CTA cluster per measurement
+// Independent outlier checks against the same (m, P): one launch of 8-CTA clusters. A small check runs on one CTA of a shared
+// cluster (ek2_check_cta), any other on a cluster of its own (ek2_body); ekf_launch_check_batch2 decides and sets `compact`.
 #define EKF_MAX_BATCH 24
 #define EKF_RES_STRIDE 32
 struct EkfCheckItem {
     const double* H; const double* f; const double* y;   // device
     int n, l;
     double Rdiag, chi2Thr, rmseThr;
-    int skipChi2, pad;
+    int skipChi2;
+    int compact;          // 1: runs on one CTA
 };
-struct EkfCheckBatch { int count; int pad; EkfCheckItem it[EKF_MAX_BATCH]; };
+struct EkfCheckBatch { int count; int compact; EkfCheckItem it[EKF_MAX_BATCH]; };   // compact: number of items with it[i].compact
 
 #define EKF_MAX_PREDICT 16
 struct EkfPredictSample {

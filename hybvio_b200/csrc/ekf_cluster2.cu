@@ -25,15 +25,29 @@ __global__ void __launch_bounds__(EK2_NT) ekf_update_cluster2_chunked_kernel(Ekf
     ek2_body<true>(a, ek2_sm, cg::this_cluster());
 }
 
-// Batched outlier checks: cluster i works on measurement i against the same state (read-only), with its own result words.
-// b.withAugment: one more cluster runs the pose augmentation that FOLLOWS the checks in the caller's sequence (aug: its argument block).
+// Item of the batch that runs the j-th check of one form (compact: on one CTA; otherwise on a cluster of its own), in item order;
+// past the last: -1 for the compact form, b.count (the augmentation) for the other
+__device__ __forceinline__ int ek2_batch_item(const EkfCheckBatch& b, int compact, int j)
+{
+    for (int i = 0; i < b.count; i++)
+        if (b.it[i].compact == compact && j-- == 0) return i;
+    return compact ? -1 : b.count;
+}
+
+// Batched outlier checks against the same state (read-only), each with its own result words (index = item). The clusters, in order:
+//   ceil(b.compact / 8) clusters whose CTA r runs the (8q + r)-th compact check on its own (ek2_check_cta: 8 checks per 8 SMs);
+//   one cluster per check that does not fit one CTA (ek2_body, as a single check);
+//   aug != a: one more cluster runs the pose augmentation that FOLLOWS the checks in the caller's sequence (aug: its argument block).
 // The checks only read (m, P) and the augmentation writes its result to the second buffers (aug.specP / aug.specM, adopted by the
 // host with a pointer swap), so the two are independent and share the launch instead of queueing behind each other.
 __global__ void __launch_bounds__(EK2_NT) ekf_check_batch_cluster2_kernel(EkfUpdateArgs a, EkfCheckBatch b, EkfUpdateArgs aug)
 {
     extern __shared__ __align__(16) double ek2_sm[];
     cg::cluster_group cluster = cg::this_cluster();
-    const int inst = blockIdx.x / EK2_C;
+    const int k = blockIdx.x / EK2_C, compactClusters = (b.compact + EK2_C - 1) / EK2_C;
+    const bool compact = k < compactClusters;
+    const int inst = compact ? ek2_batch_item(b, 1, k * EK2_C + (int)cluster.block_rank()) : ek2_batch_item(b, 0, k - compactClusters);
+    if (inst < 0) return;                                       // the last compact cluster has fewer than 8 checks
     if (inst >= b.count) a = aug;                               // (one call of the body: its code is 340 KB)
     else {
         const EkfCheckItem& it = b.it[inst];
@@ -43,9 +57,11 @@ __global__ void __launch_bounds__(EK2_NT) ekf_check_batch_cluster2_kernel(EkfUpd
         if (a.slot) a.slot += 4 * inst;
     }
     a.b.res += (size_t)EKF_RES_STRIDE * inst;
+    if (compact) { ek2_check_cta(a, ek2_sm); return; }
     a.b.cwork += (size_t)inst * 10 * a.b.N * a.b.N;           // own exchange area (Z | reduced S | partial S)
     ek2_body<false>(a, ek2_sm, cluster);
 }
+static_assert(2 * sizeof(EkfUpdateArgs) + sizeof(EkfCheckBatch) <= 4096, "ekf_check_batch_cluster2_kernel: arguments beyond 4 KB of parameter space");
 
 // Group launch (hv_ekf_group_run_device): cluster i runs args[i], an instance of any filter of the group. The blocks live in device
 // memory (hundreds of clusters do not fit the parameter space); no cluster waits for another, so a grid of many clusters runs in waves.
@@ -105,14 +121,34 @@ cudaError_t ekf_launch_update_cluster2(const EkfUpdateArgs& a, cudaStream_t s)
     return ek2_launch(ekf_update_cluster2_kernel, 1, smem, s, a);
 }
 
-cudaError_t ekf_launch_check_batch2(const EkfUpdateArgs& a, const EkfCheckBatch& b, cudaStream_t s, const EkfUpdateArgs* aug)
+// A check runs on one CTA iff its working set fits and its size n l^2 is at most EK2_CTA_CHECK_MAX. One CTA does the work of eight
+// serially: at the bench's n = 84, l = 160 (n l^2 = 2.15e6) a batch took 80 us instead of 38 us on an H100 SXM (700 W), which the
+// host-buffer entry points wait for; n = 40, l = 90 (3.2e5) and below gain. Larger checks keep a cluster of their own.
+#define EK2_CTA_CHECK_MAX (1 << 20)
+static bool ekf_check_on_one_cta(int n, int l, int N)
+{
+    return l <= N && (long long)n * l * l <= EK2_CTA_CHECK_MAX && ek2_check_cta_smem_bytes(n, l, N) + EK2_STATIC_SMEM <= EK2_SMEM_LIMIT;
+}
+
+cudaError_t ekf_launch_check_batch2(const EkfUpdateArgs& a, const EkfCheckBatch& b0, cudaStream_t s, const EkfUpdateArgs* aug)
 {
     static bool seen[64];
     if (hv_first_use_on_device(seen)) { cudaError_t e = ek2_prepare(ekf_check_batch_cluster2_kernel); if (e != cudaSuccess) return e; }
+    EkfCheckBatch b = b0;
+    b.compact = 0;
+    int clusters = aug ? 1 : 0;
     size_t smem = 0;
-    for (int i = 0; i < b.count; i++) { const size_t v = ek2_smem_bytes(b.it[i].n, b.it[i].l, a.b.N, false); if (v > smem) smem = v; }
+    for (int i = 0; i < b.count; i++) {
+        EkfCheckItem& it = b.it[i];
+        it.compact = ekf_check_on_one_cta(it.n, it.l, a.b.N) ? 1 : 0;
+        const size_t v = it.compact ? ek2_check_cta_smem_bytes(it.n, it.l, a.b.N) : ek2_smem_bytes(it.n, it.l, a.b.N, false);
+        if (v > smem) smem = v;
+        b.compact += it.compact;
+        clusters += 1 - it.compact;
+    }
+    clusters += (b.compact + EK2_C - 1) / EK2_C;
     if (aug) { const size_t v = ek2_smem_bytes(aug->n, aug->l, a.b.N, true); if (v > smem) smem = v; }
-    return ek2_launch(ekf_check_batch_cluster2_kernel, b.count + (aug ? 1 : 0), smem, s, a, b, aug ? *aug : a);
+    return ek2_launch(ekf_check_batch_cluster2_kernel, clusters, smem, s, a, b, aug ? *aug : a);
 }
 
 cudaError_t ekf_launch_group_cluster2(const EkfUpdateArgs* hArgs, const EkfUpdateArgs* dArgs, int count, cudaStream_t s)

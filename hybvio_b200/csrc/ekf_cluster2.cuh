@@ -1032,6 +1032,112 @@ __device__ __forceinline__ void ek2_body(EkfUpdateArgs& a, double* sm, Cluster c
     cluster.sync();                                   // nobody may leave while its shared memory can still be read
 }
 
+// ---- one outlier check on ONE CTA (the compact clusters of ekf_check_batch_cluster2_kernel) --------------------------------------
+// A check needs chi2 only, and chi2 needs S = H P[0:l, 0:l] H' + R and v, not HP over all N columns nor the downdate. This body forms
+// S from the cluster's own column blocks J_c (c = 0 .. 7), one after the other in one CTA: stage P[0:l, J_c within [0, l)], HP_c with
+// the call of phase A, the partial S_c with the call of phase B, s += S_c in the order c = 0 .. 7 from +0.0 (the order of both
+// reductions of ek2_body; a block at or beyond l adds +0.0 there, which cannot change a sum that starts at +0.0, so it is skipped),
+// then + R on the diagonal. The elimination runs on [S | v] only: every entry of its products depends on its own row and column
+// operands and the k order alone, so z_v and therefore every result word are bitwise those of ek2_body. The batch's checks carry no
+// device-side gates and no second noise level (check_items). Shared memory: scratch | H (n x l, ld n) | tableau rows [S | v | HP_c]
+// (ld W, as ek2_geom's) | P block (l x B, ld LDP).
+struct Ek2CheckGeom { int B, W, LDP, X, T; };
+#define EK2_CTA_SCRATCH (EK2_LINV_DOUBLES + 4)         // L_jj^-1 (2 x 64) | rmse, chi2 | pivot flag (+ pad: H starts 16-byte aligned)
+__host__ __device__ inline Ek2CheckGeom ek2_check_geom(int n, int l, int N)
+{
+    Ek2CheckGeom g;
+    g.B = (N + EK2_C - 1) / EK2_C;
+    g.W = ek2_pad4mod16(n + 1 + g.B);
+    g.LDP = ek2_pad4mod16(l);
+    g.X = (n * l + 1) & ~1;
+    g.T = (n * g.W + 1) & ~1;
+    return g;
+}
+__host__ __device__ inline size_t ek2_check_cta_smem_bytes(int n, int l, int N)
+{
+    const Ek2CheckGeom g = ek2_check_geom(n, l, N);
+    return ((size_t)EK2_CTA_SCRATCH + g.X + g.T + (size_t)g.LDP * g.B) * sizeof(double);
+}
+
+#ifdef HV_EMU
+#define EK2_NOINLINE inline
+#else
+#define EK2_NOINLINE __noinline__             // its own register allocation: inlined beside ek2_body, the batch kernel spills
+#endif
+__device__ EK2_NOINLINE void ek2_check_cta(const EkfUpdateArgs& a, double* sm)
+{
+    const int tid = threadIdx.x, lane = tid & 31, wrp = tid >> 5;
+    const int N = a.b.N, n = a.n, l = a.l;
+    const Ek2CheckGeom g = ek2_check_geom(n, l, N);
+    const int W = g.W, B = g.B, LDP = g.LDP;
+    double* const s_linv = sm;
+    double* const s_scalar = sm + EK2_LINV_DOUBLES;
+    volatile int* const s_bad = (volatile int*)(sm + EK2_LINV_DOUBLES + 2);
+    double* const Hs = sm + EK2_CTA_SCRATCH;
+    double* const T = Hs + g.X;
+    double* const PB = T + g.T;
+    ek2_pdl_launch_dependents();                      // (see ek2_body)
+    if (!a.lateH) ek2_copy8(Hs, a.H, n * l, tid);
+    ek2_pdl_wait();
+    if (a.lateH) ek2_copy8(Hs, a.H, n * l, tid);
+    __syncthreads();
+    for (int i = tid; i < n; i += EK2_NT) {
+        const double yi = a.y ? a.y[i] : a.ysmall[i];
+        double fi = 0.0;
+        if (a.f) fi = a.f[i];
+        else for (int k = 0; k < l; k++) fi += Hs[i + (size_t)k * n] * a.b.m[k];
+        T[(size_t)i * W + n] = yi - fi;
+    }
+    for (int e = tid; e < n * n; e += EK2_NT) T[(size_t)(e / n) * W + (e % n)] = 0.0;
+    __syncthreads();
+    if (a.rmseThr >= 0.0) {                           // ekf.cpp:797-801
+        if (tid == 0) { double ss = 0.0; for (int i = 0; i < n; i++) { const double v = T[(size_t)i * W + n]; ss += v * v; } s_scalar[0] = sqrt(ss / n); }
+        __syncthreads();
+        if (s_scalar[0] > a.rmseThr) { if (tid == 0) ekf_report(a, 2.0, 0.0, 0.0); return; }
+    }
+    if (a.skipChi2) { if (tid == 0) ekf_report(a, 0.0, 0.0, 0.0); return; }
+
+    for (int c = 0; c < EK2_C; c++) {
+        const int J0 = c * B, kc = min(B, l - J0);    // (l <= N: the block's columns below l)
+        if (kc <= 0) break;
+        const double* src = a.b.P + (size_t)J0 * N;
+        const int count = l * kc;
+        for (int base = 0; base < count; base += 8 * EK2_NT) {
+            double r[8];
+#pragma unroll
+            for (int u = 0; u < 8; u++) { const int t = base + u * EK2_NT + tid, j = t / l; r[u] = t < count ? src[(t - j * l) + (size_t)j * N] : 0.0; }
+#pragma unroll
+            for (int u = 0; u < 8; u++) { const int t = base + u * EK2_NT + tid, j = t / l; if (t < count) PB[(t - j * l) + (size_t)j * LDP] = r[u]; }
+        }
+        __syncthreads();
+        ek2_dmma_gemm(n, kc, l, wrp, lane, Hs, 1, n, PB, 1, LDP,
+                      [](int, int) { return 0.0; },
+                      [&](int i, int j, double v0, double v1) { T[(size_t)i * W + n + 1 + j] = v0; if (j + 1 < kc) T[(size_t)i * W + n + 2 + j] = v1; });
+        __syncthreads();
+        ek2_dmma_gemm<true>(n, n, kc, wrp, lane, T + n + 1, W, 1, Hs + (size_t)J0 * n, n, 1,
+                            [](int, int) { return 0.0; },
+                            [&](int i, int j, double v0, double v1) { T[(size_t)i * W + j] += v0; if (j + 1 < n) T[(size_t)i * W + j + 1] += v1; });
+        __syncthreads();
+    }
+    for (int i = tid; i < n; i += EK2_NT) T[(size_t)i * W + i] += a.Rdiag;
+    __syncthreads();
+    if (!ek2_block_eliminate(T, W, n, n + 1, wrp, lane, s_linv, s_bad)) {
+        if (tid == 0) ekf_report(a, 1.0, 0.0, 1.0);
+        return;
+    }
+    __syncthreads();
+    if (wrp == 0) {                                   // as ek2_body: lane-strided sums, fixed shuffle tree
+        double t = 0.0;
+        for (int k = lane; k < n; k += 32) { const double z = T[(size_t)k * W + n]; t += z * z; }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) t += __shfl_sync(0xffffffffu, t, lane ^ o);
+        if (lane == 0) s_scalar[1] = a.noiseScale * t;
+    }
+    __syncthreads();
+    const double chi2 = s_scalar[1];
+    if (tid == 0) ekf_report(a, chi2 > a.chi2Thr ? 3.0 : 0.0, chi2, 0.0);
+}
+
 // Cluster `inst` of a group launch (ekf_group_cluster2_kernel): its own argument block, fully resolved by the host (filter buffers,
 // exchange area, result words, second buffers), read from device memory. Clusters of one launch share nothing.
 template <class Cluster>
