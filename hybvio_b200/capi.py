@@ -486,8 +486,12 @@ class Ingest:
         check(self.lib.hv_ingest_set_remap(self.h_, _ptr(np.ascontiguousarray(table))), "hv_ingest_set_remap")
 
     def frame(self, img, pyr, coeff=None, want_gray=True):
-        img = np.ascontiguousarray(img, np.uint8)
+        """img: (h, w) gray or (h, w, channels) uint8. A view whose rows are dense (e.g. a crop of a wider buffer) is passed with its own
+        row stride, as the C adapters pass an image's bytesPerRow(); any other layout is copied first."""
+        img = np.asarray(img)
         channels = 1 if img.ndim == 2 else img.shape[2]
+        if img.dtype != np.uint8 or img.strides[1:] != ((channels, 1) if img.ndim == 3 else (1,)) or img.strides[0] < img.shape[1] * channels:
+            img = np.ascontiguousarray(img, np.uint8)
         out = np.zeros((self.h, self.w), np.uint8) if want_gray else None
         cf = None if coeff is None else np.ascontiguousarray(list(coeff) + [0.0] * (4 - len(coeff)), np.float64)
         check(self.lib.hv_ingest_frame(self.h_, _ptr(img), img.strides[0], channels, None if cf is None else _ptr(cf), pyr.h, None if out is None else _ptr(out)),

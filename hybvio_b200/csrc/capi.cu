@@ -233,8 +233,8 @@ int hv_pyr_build_batch(hv_pyr* const* pyrs, const uint8_t* const* gray, const si
         if (srcIsDevice) {      // frame already in HBM: the kernel reads it in place and fills level 0 itself
             src[i] = gray[i]; srcPitch[i] = (int)strides[i];
         } else {                // the frame lands directly in the level-0 buffer: level 0 of the pyramid IS the input image
-            if (strides[i] == (size_t)L0.gpitch)
-                HV_CUDA(cudaMemcpyAsync(L0.gray, gray[i], (size_t)L0.gpitch * p->h, cudaMemcpyHostToDevice, c->stream));
+            if (strides[i] == (size_t)L0.gpitch)     // one 1-D copy up to the last pixel (the caller's buffer may end there)
+                HV_CUDA(cudaMemcpyAsync(L0.gray, gray[i], (size_t)L0.gpitch * (p->h - 1) + p->w, cudaMemcpyHostToDevice, c->stream));
             else
                 HV_CUDA(cudaMemcpy2DAsync(L0.gray, L0.gpitch, gray[i], strides[i], (size_t)p->w, (size_t)p->h, cudaMemcpyHostToDevice, c->stream));
             src[i] = nullptr; srcPitch[i] = 0;
@@ -816,7 +816,8 @@ struct hv_ingest {
     hv_ctx* ctx = nullptr;
     int w = 0, h = 0;
     uint8_t* d_raw = nullptr; size_t rawBytes = 0;     // the frame as it arrived (device)
-    uint8_t* d_gray = nullptr;                          // gray before the remap (w x h, pitch w rounded up to 4)
+    uint8_t* d_gray = nullptr;                          // gray before the remap (w x h, pitch w: a remap tap right of the last column
+                                                        // reads the next row's first pixel, as the reference's contiguous image does)
     HvRemapEntry* d_table = nullptr;
 };
 
@@ -826,8 +827,7 @@ int hv_ingest_create(hv_ctx* c, int w, int h, hv_ingest** out)
     HV_CUDA(cudaSetDevice(c->device));
     hv_ingest* g = new hv_ingest;
     g->ctx = c; g->w = w; g->h = h;
-    const size_t gp = (size_t)((w + 3) & ~3);
-    cudaError_t e = cudaMalloc(&g->d_gray, gp * h);
+    cudaError_t e = cudaMalloc(&g->d_gray, (size_t)w * h);
     if (e != cudaSuccess) { delete g; hv_set_error("hv_ingest_create: %s", cudaGetErrorString(e)); return HV_ERR_OOM; }
     *out = g;
     return HV_OK;
@@ -861,20 +861,19 @@ int hv_ingest_frame(hv_ingest* g, const uint8_t* src, size_t stride, int channel
     HV_CUDA(cudaSetDevice(c->device));
     const int w = g->w, h = g->h;
     const HvLevel& L0 = dst->desc.lv[0];
-    const int gp = (w + 3) & ~3;
     const bool colour = channels > 1, remap = g->d_table != nullptr;
     if (!colour && !remap) {                                     // plain gray frame: exactly hv_pyr_build
         int rc = hv_pyr_build(dst, src, stride);
         if (rc != HV_OK) return rc;
     } else {
-        const size_t need = stride * h;
+        const size_t need = stride * (h - 1) + (size_t)w * channels;                               // up to the last pixel: no byte past it
         if (need > g->rawBytes) { cudaStreamSynchronize(c->stream); cudaFree(g->d_raw); g->d_raw = nullptr; g->rawBytes = 0; HV_CUDA(cudaMalloc(&g->d_raw, need)); g->rawBytes = need; }
         HV_CUDA(cudaMemcpyAsync(g->d_raw, src, need, cudaMemcpyHostToDevice, c->stream));          // the only trip of the frame over PCIe
         const uint8_t* cur = g->d_raw; int curPitch = (int)stride;
         if (colour) {
             float cf[4] = {0.299f, 0.587f, 0.114f, 0.0f};                                          // image.cpp:360-366
             if (coeff) for (int i = 0; i < 4; i++) cf[i] = i < channels ? (float)coeff[i] : 0.0f;
-            uint8_t* out = remap ? g->d_gray : L0.gray; const int op = remap ? gp : L0.gpitch;
+            uint8_t* out = remap ? g->d_gray : L0.gray; const int op = remap ? w : L0.gpitch;
             HV_CUDA(hv_launch_gray(cur, curPitch, channels, w, h, cf, out, op, c->stream));
             c->launches += 1;
             cur = out; curPitch = op;

@@ -17,26 +17,38 @@ def have_ref():
     return os.path.exists(REF_SO)
 
 
+def _rows(img, channels):
+    """(image, row stride in bytes): a uint8 view whose rows are dense keeps its own stride (the reference reads its image as it lies in
+    memory, padding bytes after a row included); any other layout is copied."""
+    img = np.asarray(img)
+    dense = (channels, 1) if img.ndim == 3 else (1,)
+    if img.dtype != np.uint8 or img.strides[1:] != dense or img.strides[0] < img.shape[1] * channels:
+        img = np.ascontiguousarray(img, np.uint8)
+    return img, img.strides[0]
+
+
 class OracleIngest:
     def __init__(self):
         self.lib = ctypes.CDLL(ORACLE_SO)
 
     def gray(self, img, coeff=GRAY_COEFF):
-        img = np.ascontiguousarray(img, np.uint8)
-        h, w, c = img.shape
+        h, w, c = np.shape(img)
+        img, stride = _rows(img, c)
         cf = np.array([np.float32(x) for x in coeff[:c]], np.float32)      # the reference stores the coefficients as fp32
         out = np.zeros((h, w), np.uint8)
-        self.lib.orc_gray(img.ctypes.data_as(ctypes.c_void_p), ctypes.c_int(w * c), ctypes.c_int(c), ctypes.c_int(w), ctypes.c_int(h),
+        self.lib.orc_gray(img.ctypes.data_as(ctypes.c_void_p), ctypes.c_int(stride), ctypes.c_int(c), ctypes.c_int(w), ctypes.c_int(h),
                           cf.ctypes.data_as(ctypes.c_void_p), out.ctypes.data_as(ctypes.c_void_p))
         return out
 
     def remap(self, img, table):
-        img = np.ascontiguousarray(img, np.uint8)
-        h, w = img.shape
+        """A tap right of the last column reads the first byte after the row in memory: for a view into a wider buffer that is the view's
+        padding, for a contiguous image the first pixel of the next row."""
+        h, w = np.shape(img)
+        img, stride = _rows(img, 1)
         table = np.ascontiguousarray(table, REMAP_DTYPE)
         assert table.size == w * h and REMAP_DTYPE.itemsize == 12
         out = np.zeros((h, w), np.uint8)
-        self.lib.orc_remap(img.ctypes.data_as(ctypes.c_void_p), ctypes.c_int(w), ctypes.c_int(w), ctypes.c_int(h), table.ctypes.data_as(ctypes.c_void_p),
+        self.lib.orc_remap(img.ctypes.data_as(ctypes.c_void_p), ctypes.c_int(stride), ctypes.c_int(w), ctypes.c_int(h), table.ctypes.data_as(ctypes.c_void_p),
                            out.ctypes.data_as(ctypes.c_void_p))
         return out
 
