@@ -89,6 +89,15 @@ class SubpixJob(ctypes.Structure):
 
 CORNER_BATCH_MAX = 64   # HV_CORNER_BATCH_MAX
 
+
+class IngestJob(ctypes.Structure):
+    """hv_ingest_job: one frame of hv_ingest_frames (see ingest_job)"""
+    _fields_ = [("ing", c_void_p), ("src", c_void_p), ("stride_bytes", c_size_t), ("channels", c_int), ("coeff", c_void_p),
+                ("dst", c_void_p), ("gray_out", c_void_p)]
+
+
+INGEST_BATCH_MAX = 128  # HV_INGEST_BATCH_MAX
+
 _lib = None
 
 
@@ -126,6 +135,7 @@ def load():
     lib.hv_ingest_destroy.argtypes = [c_void_p]
     lib.hv_ingest_set_remap.argtypes = [c_void_p, c_void_p]
     lib.hv_ingest_frame.argtypes = [c_void_p, c_void_p, c_size_t, c_int, c_void_p, c_void_p, c_void_p]
+    lib.hv_ingest_frames.argtypes = [ctypes.POINTER(IngestJob), c_int, c_int]
     lib.hv_gftt_cells.argtypes = [c_void_p, c_int, ctypes.POINTER(c_int), ctypes.POINTER(c_int)]
     lib.hv_gftt_detect.argtypes = [c_void_p, c_void_p, c_int, c_int, ctypes.c_float, c_void_p]
     lib.hv_gftt_detect_device.argtypes = [c_void_p, c_void_p, c_int, c_int, ctypes.c_float, c_void_p]
@@ -306,6 +316,13 @@ class Context:
         S = (c_size_t * n)(*[_stride0(im) for im in images])
         check(self.lib.hv_pyr_build_batch(P, G, S, n, 1 if device else 0), "hv_pyr_build_batch")
 
+    def ingest_frames(self, jobs, device=False):
+        """hv_ingest_frames: Ingest.frame for every job (see ingest_job) with the launches of one; asynchronous (synchronise before
+        reading a gray_out). device: every source is a CUDA tensor, read in place; otherwise every source is host memory."""
+        assert all(j.on_device == bool(device) for j in jobs), "sources must all be on the device (device=True) or all on the host"
+        J = (IngestJob * len(jobs))(*jobs)
+        check(self.lib.hv_ingest_frames(J, len(jobs), 1 if device else 0), "hv_ingest_frames")
+
     # ---- tracker::OpticalFlow::compute
     def lk_track(self, prev, nxt, prev_xy, next_xy=None, max_iter=20, eps=0.03, min_eig=1e-3):
         """Host-buffer LK. Returns (next_xy float32 (n,2), status uint8 (n,), track_status int32 (n,))."""
@@ -379,6 +396,39 @@ def subpix_job(pyr, d_xy, n=None):
     """A SubpixJob: the first n (all) points of a contiguous (m, 2) float32 CUDA tensor on level 0 of pyr."""
     _check_cuda_buffer(d_xy)
     return SubpixJob(pyr.h.value, _ptr(d_xy), d_xy.numel() // 2 if n is None else n)
+
+
+def _dense_rows(img):
+    """A host image as Ingest.frame passes it: a uint8 view whose rows are dense keeps its own row stride, any other layout is copied."""
+    img = np.asarray(img)
+    channels = 1 if img.ndim == 2 else img.shape[2]
+    if img.dtype != np.uint8 or img.strides[1:] != ((channels, 1) if img.ndim == 3 else (1,)) or img.strides[0] < img.shape[1] * channels:
+        img = np.ascontiguousarray(img, np.uint8)
+    return img, channels
+
+
+def _coeff_array(coeff):
+    return None if coeff is None else np.ascontiguousarray(list(coeff) + [0.0] * (4 - len(coeff)), np.float64)
+
+
+def ingest_job(ing, img, pyr, coeff=None, gray_out=None):
+    """An IngestJob: frame img ((h, w) gray or (h, w, channels) uint8) through `ing` into `pyr`. img is a numpy array (host; a view whose
+    rows are dense keeps its own row stride, as Ingest.frame passes it) or a torch uint8 tensor with dense rows (a CUDA tensor for
+    Context.ingest_frames(..., device=True), else host memory, pinned for an asynchronous copy). gray_out: None or a (h, w) uint8 C-contiguous
+    numpy array that receives the ingested image. The job keeps img, the coefficients and gray_out alive."""
+    if isinstance(img, np.ndarray) or not hasattr(img, "data_ptr"):
+        img, channels = _dense_rows(img)
+        on_device = False
+    else:
+        channels = 1 if img.dim() == 2 else img.shape[2]
+        assert img.dtype.itemsize == 1 and img.stride()[1:] == ((channels, 1) if img.dim() == 3 else (1,)), "rows must be dense"
+        on_device = img.is_cuda
+    if gray_out is not None:
+        assert gray_out.dtype == np.uint8 and gray_out.shape == (ing.h, ing.w) and gray_out.flags.c_contiguous
+    cf = _coeff_array(coeff)
+    job = IngestJob(ing.h_.value, _ptr(img), _stride0(img), channels, _ptr(cf), pyr.h.value, _ptr(gray_out))
+    job.on_device, job.keep = on_device, (img, cf, gray_out)
+    return job
 
 
 def gftt_select_capacity(nkp, mask_radius, max_tracks):
@@ -488,12 +538,9 @@ class Ingest:
     def frame(self, img, pyr, coeff=None, want_gray=True):
         """img: (h, w) gray or (h, w, channels) uint8. A view whose rows are dense (e.g. a crop of a wider buffer) is passed with its own
         row stride, as the C adapters pass an image's bytesPerRow(); any other layout is copied first."""
-        img = np.asarray(img)
-        channels = 1 if img.ndim == 2 else img.shape[2]
-        if img.dtype != np.uint8 or img.strides[1:] != ((channels, 1) if img.ndim == 3 else (1,)) or img.strides[0] < img.shape[1] * channels:
-            img = np.ascontiguousarray(img, np.uint8)
+        img, channels = _dense_rows(img)
         out = np.zeros((self.h, self.w), np.uint8) if want_gray else None
-        cf = None if coeff is None else np.ascontiguousarray(list(coeff) + [0.0] * (4 - len(coeff)), np.float64)
+        cf = _coeff_array(coeff)
         check(self.lib.hv_ingest_frame(self.h_, _ptr(img), img.strides[0], channels, None if cf is None else _ptr(cf), pyr.h, None if out is None else _ptr(out)),
               "hv_ingest_frame")
         self.ctx.sync()

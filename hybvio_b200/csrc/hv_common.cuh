@@ -160,3 +160,18 @@ cudaError_t hv_launch_subpix_batch(const SubpixBatchArgs& b, int njobs, cudaStre
 struct HvRemapEntry { short x0, y0; float xfrac, yfrac; };      // 12 bytes per output pixel (hv_remap_entry of the C ABI)
 cudaError_t hv_launch_gray(const uint8_t* src, int srcPitch, int channels, int w, int h, const float coeff[4], uint8_t* dst, int dstPitch, cudaStream_t s);
 cudaError_t hv_launch_remap(const uint8_t* src, int srcPitch, int w, int h, const HvRemapEntry* table, uint8_t* dst, int dstPitch, cudaStream_t s);
+
+// Frames that need colour conversion and / or a remap, HV_CORNER_BATCH_MAX per launch (hv_ingest_frames)
+struct IngestJob {
+    const uint8_t* src; int srcPitch, channels;     // channels > 1: colour -> gray
+    float coeff[4];                                 // resolved as hv_ingest_frame resolves them
+    const HvRemapEntry* table;                      // NULL: no remap
+    uint8_t* dst; int dstPitch;                     // level 0 of the pyramid
+    int w, h;
+};
+struct IngestBatchArgs {
+    IngestJob job[HV_CORNER_BATCH_MAX];
+    int first[HV_CORNER_BATCH_MAX + 1];             // first CTA of job j: prefix sum of ceil(w / 256) * h; first[njobs ..] = the grid
+};
+static_assert(sizeof(IngestBatchArgs) <= HV_KERNEL_PARAM_MAX, "ingest batch arguments exceed the kernel-parameter space");
+cudaError_t hv_launch_ingest_batch(const IngestBatchArgs& b, int njobs, cudaStream_t s);

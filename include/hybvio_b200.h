@@ -227,6 +227,31 @@ int hv_ingest_create(hv_ctx* ctx, int width, int height, hv_ingest** out);
 int hv_ingest_destroy(hv_ingest* ing);
 int hv_ingest_set_remap(hv_ingest* ing, const hv_remap_entry* table);     /* width * height entries, host; NULL removes the table */
 int hv_ingest_frame(hv_ingest* ing, const uint8_t* src, size_t stride_bytes, int channels, const double* coeff, hv_pyr* dst, uint8_t* gray_out);
+/* hv_ingest_frames: hv_ingest_frame for up to HV_INGEST_BATCH_MAX frames (a stereo pair, or the pairs of many sessions sharing the
+ * context) with the launches of one. Every job leaves the same bytes as hv_ingest_frame(job.ing, job.src, ...) would: every level of
+ * dst (gray and gradients) and gray_out. Asynchronous, on the context's stream.
+ *   src_is_device != 0: every src is a device pointer, read in place (no copy; e.g. a frame decoded on the GPU). Otherwise every src is
+ *     host memory, copied once into its own hv_ingest's staging buffer up to the last pixel (no byte past it), as hv_ingest_frame does;
+ *     it must stay valid until the next synchronising call.
+ *   Jobs that need colour conversion or a remap run in ceil(k / 64) launches of one kernel (k such jobs). Gray jobs without a table skip
+ *   it, as hv_ingest_frame does: a host source is copied into level 0, a device source is read in place by the pyramid kernel, as in
+ *   hv_pyr_build_batch(..., 1). The pyramids are then built with one pyramid launch per 32 frames of one level-0 size (pyramids of
+ *   different depth share a launch). A rectified stereo pair takes 2 launches, and so do 16 such pairs of one size.
+ * Errors, checked for every job before anything is copied or launched (a refused call leaves every pyramid and gray_out untouched and
+ * the context's launch count unchanged): HV_ERR_INVALID for njobs outside 1..HV_INGEST_BATCH_MAX; a NULL jobs, ing, src or dst;
+ * channels outside 1..4 or a stride below w * channels; an ing or dst of another context than jobs[0].ing, or a dst whose size differs
+ * from its ing; the same hv_ingest twice (it has one staging buffer and one table) or the same pyramid twice; a device source whose
+ * bytes [src, src + stride * (h - 1) + w * channels) overlap the memory of any job's pyramid (the call writes it while it reads the
+ * source). */
+#define HV_INGEST_BATCH_MAX 128            /* 64 stereo sessions, matching the 64-session corner and EKF batches */
+typedef struct hv_ingest_job {
+    hv_ingest* ing;                        /* size and remap table (may have none) */
+    const uint8_t* src; size_t stride_bytes; int channels;
+    const double* coeff;                   /* NULL: 0.299, 0.587, 0.114, 0 (as hv_ingest_frame) */
+    hv_pyr* dst;
+    uint8_t* gray_out;                     /* host, optional, w x h tightly packed */
+} hv_ingest_job;
+int hv_ingest_frames(const hv_ingest_job* jobs, int njobs, int src_is_device);
 
 /* ---------------------------------------------------------------- EKF ----------------------------------- */
 /* Replaces odometry::EKF / EKFImplementation (src/odometry/ekf.hpp:62-174, ekf.cpp). State m (N) and
