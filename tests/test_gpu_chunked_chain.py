@@ -13,6 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 import kalman_ref as K  # noqa: E402
 import tri_common  # noqa: E402
+import visual_update_ref as V  # noqa: E402
 from test_gpu_track_model import sequential_reference_flow  # noqa: E402
 
 pytestmark = pytest.mark.gpu
@@ -137,13 +138,18 @@ def test_chunked_update_matches_extended_precision_reference(hv, trail, ms):
     st, c2 = K.check(P0, H, f, y, chi_r, ns)
     assert st == 0
     ref = K.update(m0, P0, H, f, y, vis_r, ns, trail)
+    chunks = V.chain_chunks(84, H.shape[1], e.N)
+    ref_c = V.update(m0, P0, H, f, y, vis_r, ns, trail, chunks)
     got, succ = e.visual_tracks([track], chi_r, vis_r, max_successful_updates=1)
     assert succ == 1 and got[0]["updated"] and got[0]["outlier_status"] == 0
     t_chk, t_upd = K.tau(84, K.kappa_S(P0, H, chi_r, ns)), K.tau(84, K.kappa_S(P0, H, vis_r, ns))
-    em, eP = K.errors(ref[0], ref[1], *e.download())
+    m1, P1 = e.download()
+    em, eP = K.errors(ref[0], ref[1], m1, P1)
     rc = K.chi2_error(c2, got[0]["chi2"]) / t_chk
-    print(f"N={e.N}: error / tau = {max(em, eP) / t_upd:.3g} (m, P), {rc:.3g} (chi2)")
+    rv, where = V.worst(ref_c, m1, P1, trail, ms)
+    print(f"N={e.N}: error / tau = {max(em, eP) / t_upd:.3g} (m, P), {rc:.3g} (chi2); {chunks} chunks, per-entry ratio {rv:.3g} at {where}")
     assert max(em, eP) <= t_upd and rc <= 1.0
+    assert rv <= 1.0, where
     e.close()
 
 

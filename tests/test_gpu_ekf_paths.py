@@ -13,6 +13,7 @@ sys.path.insert(0, os.path.dirname(__file__))
 import ekf_common as C
 import ekf_script
 import kalman_ref as K
+import visual_update_ref as V
 
 pytestmark = pytest.mark.gpu
 R, R_CHECK, NS = 0.05, 0.07, 100.0
@@ -43,6 +44,7 @@ class Case:
         self.kappa = K.kappa_S(self.P, self.H, R, NS)
         self.tau = K.tau(n, self.kappa)
         self.ref = K.update(self.m, self.P, self.H, self.f, self.y, R, NS, trail)
+        self.ref_c = V.update(self.m, self.P, self.H, self.f, self.y, R, NS, trail)
         self.checkable = n <= K.CHI2_MAX_N
         if self.checkable:
             thr = K.chi2inv95(n)
@@ -52,7 +54,7 @@ class Case:
             assert self.ref_in[0] == 0 and self.ref_in2[0] == 0 and self.ref_out[0] == 3
             for _, c2 in (self.ref_in, self.ref_in2, self.ref_out):           # no decision within tau of the threshold
                 assert abs(float(c2) - thr) > 1e-6 * thr
-        self.worst = 0.0
+        self.worst = self.worst_c = 0.0
 
     def state_ratio(self, got):
         em, eP = K.errors(self.ref[0], self.ref[1], got[0], got[1])
@@ -62,6 +64,9 @@ class Case:
         r = self.state_ratio(got)
         self.worst = max(self.worst, r)
         assert r <= 1.0, f"{what}: error / tau = {r:.3g}"
+        rc, where = V.worst(self.ref_c, got[0], got[1], self.trail, self.ms)
+        self.worst_c = max(self.worst_c, rc)
+        assert rc <= 1.0, f"{what}: per-entry ratio {rc:.3g} at {where}"
 
     def assert_check(self, st, c2, ref, what):
         assert st == ref[0], f"{what}: status {st} != {ref[0]}"
@@ -154,7 +159,7 @@ def test_update_path_matches_extended_precision_reference(hv, oracle_lk, trail, 
     e.close()
     path = K.kernel_path(n, l, c.N)
     print(f"\nPATH N={c.N} n={n} l={l} {'/'.join(path)} (misaligned H: {'/'.join(K.kernel_path(n, l, c.N, h_aligned=False))}) "
-          f"kappa={c.kappa:.3g} worst error / tau = {c.worst:.3g}")
+          f"kappa={c.kappa:.3g} worst error / tau = {c.worst:.3g}, worst per-entry ratio = {c.worst_c:.3g}")
 
 
 @pytest.mark.parametrize("trail,ms", K.CONFIGS)
