@@ -87,6 +87,11 @@ class SubpixJob(ctypes.Structure):
     _fields_ = [("pyr", c_void_p), ("d_xy", c_void_p), ("n", c_int)]
 
 
+class FastJob(ctypes.Structure):
+    """hv_fast_job: one session's pyramid and outputs in the batched FAST detection (see fast_job)"""
+    _fields_ = [("pyr", c_void_p), ("d_xy", c_void_p), ("d_response", c_void_p), ("capacity", c_int), ("d_count", c_void_p)]
+
+
 CORNER_BATCH_MAX = 64   # HV_CORNER_BATCH_MAX
 
 
@@ -146,6 +151,9 @@ def load():
     lib.hv_gftt_detect_batch_device.argtypes = [c_void_p, ctypes.POINTER(CornerJob), c_int, c_int, c_int, ctypes.c_float]
     lib.hv_gftt_select_batch_device.argtypes = [c_void_p, ctypes.POINTER(CornerJob), c_int]
     lib.hv_subpix_refine_batch_device.argtypes = [c_void_p, ctypes.POINTER(SubpixJob), c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_double]
+    lib.hv_fast_detect.argtypes = [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p]
+    lib.hv_fast_detect_device.argtypes = lib.hv_fast_detect.argtypes
+    lib.hv_fast_detect_batch_device.argtypes = [c_void_p, ctypes.POINTER(FastJob), c_int, c_int, c_int]
     _bind_ekf(lib)
     _lib = lib
     return lib
@@ -362,6 +370,11 @@ class Context:
         check(self.lib.hv_subpix_refine_batch_device(self.h, J, len(jobs), win[0], win[1], zero_zone[0], zero_zone[1],
                                                      criteria[0], criteria[1], criteria[2]), "hv_subpix_refine_batch_device")
 
+    def fast_detect_batch_device(self, jobs, threshold=10, nonmax=True):
+        """hv_fast_detect_batch_device: cv::FAST on level 0 of every job's pyramid (see fast_job), two launches; asynchronous."""
+        J = (FastJob * len(jobs))(*jobs)
+        check(self.lib.hv_fast_detect_batch_device(self.h, J, len(jobs), threshold, 1 if nonmax else 0), "hv_fast_detect_batch_device")
+
     def lk_track_device(self, prev, nxt, d_prev, d_next, d_status, d_ts, n, use_initial, max_iter=20, eps=0.03, min_eig=1e-3):
         check(self.lib.hv_lk_track_device(self.h, prev.h, nxt.h, _ptr(d_prev), _ptr(d_next), _ptr(d_status), _ptr(d_ts), n,
                                           1 if use_initial else 0, max_iter, eps, min_eig), "hv_lk_track_device")
@@ -396,6 +409,14 @@ def subpix_job(pyr, d_xy, n=None):
     """A SubpixJob: the first n (all) points of a contiguous (m, 2) float32 CUDA tensor on level 0 of pyr."""
     _check_cuda_buffer(d_xy)
     return SubpixJob(pyr.h.value, _ptr(d_xy), d_xy.numel() // 2 if n is None else n)
+
+
+def fast_job(pyr, d_xy, d_count, d_response=None):
+    """A FastJob on contiguous CUDA tensors: d_xy (capacity, 2) float32, d_count (1,) int32, d_response (capacity,) float32 or None.
+    The tensors must outlive the call that uses the job."""
+    for t in (d_xy, d_count) + (() if d_response is None else (d_response,)):
+        _check_cuda_buffer(t)
+    return FastJob(pyr.h.value, _ptr(d_xy), _ptr(d_response), d_xy.numel() // 2, _ptr(d_count))
 
 
 def _dense_rows(img):
@@ -512,6 +533,30 @@ class Pyramid:
         n = d_xy.numel() // 2
         check(self.lib.hv_subpix_refine_device(self.ctx.h, self.h, _ptr(d_xy), n, win[0], win[1], zero_zone[0], zero_zone[1],
                                                criteria[0], criteria[1], criteria[2]), "hv_subpix_refine_device")
+
+    def fast_detect(self, threshold=10, nonmax=True, capacity=None):
+        """cv::FAST (TYPE_9_16) on the level-0 image of this pyramid. Returns (xy (n, 2) float32, response (n,) float32) in OpenCV's
+        order: every keypoint, or the first `capacity` of them when a capacity is given (a second call fetches the rest when the
+        first guess of 4096 was too small)."""
+        cap = 4096 if capacity is None else capacity
+        while True:
+            xy = np.zeros((max(cap, 1), 2), np.float32)
+            resp = np.zeros(max(cap, 1), np.float32)
+            n = c_int(0)
+            check(self.lib.hv_fast_detect(self.ctx.h, self.h, threshold, 1 if nonmax else 0, _ptr(xy), _ptr(resp), cap, ctypes.byref(n)),
+                  "hv_fast_detect")
+            if capacity is not None or n.value <= cap:
+                m = min(n.value, cap)
+                return xy[:m].copy(), resp[:m].copy()
+            cap = n.value
+
+    def fast_detect_device(self, d_xy, d_count, d_response=None, threshold=10, nonmax=True):
+        """hv_fast_detect_device on contiguous CUDA tensors: d_xy (capacity, 2) float32, d_count (1,) int32, d_response (capacity,)
+        float32 or None; asynchronous on the context's stream."""
+        for t in (d_xy, d_count) + (() if d_response is None else (d_response,)):
+            _check_cuda_buffer(t)
+        check(self.lib.hv_fast_detect_device(self.ctx.h, self.h, threshold, 1 if nonmax else 0, _ptr(d_xy), _ptr(d_response),
+                                             d_xy.numel() // 2, _ptr(d_count)), "hv_fast_detect_device")
 
     def release(self):
         if self.h:

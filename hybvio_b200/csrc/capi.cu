@@ -77,6 +77,7 @@ int hv_ctx_destroy(hv_ctx* c)
     if (c->h_stage) cudaFreeHost(c->h_stage);
     if (c->d_done) cudaFree(c->d_done);
     if (c->d_selectScratch) cudaFree(c->d_selectScratch);
+    if (c->d_fastScratch) cudaFree(c->d_fastScratch);
     if (c->d_ekfStage) cudaFree(c->d_ekfStage);
     for (int i = 0; i < HV_EKF_STAGES; i++) {
         if (c->h_ekfStage[i]) cudaFreeHost(c->h_ekfStage[i]);
@@ -808,6 +809,113 @@ int hv_subpix_refine_batch_device(hv_ctx* c, const hv_subpix_job* jobs, int njob
     HV_CUDA(cudaSetDevice(c->device));
     HV_CUDA(hv_launch_subpix_batch(b, njobs, c->stream));
     c->launches += 1;
+    return HV_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ FAST corner detection (N2)
+// Checks one job (its pointers and counts) and fills everything but the scratch; *scratch = the bytes of masks and tile counts it needs.
+static int fast_args(const char* who, hv_ctx* c, hv_pyr* pyr, int threshold, int nonmax, float* xy, float* response, int capacity, int* count,
+                     FastArgs& a, size_t* scratch)
+{
+    if (!c || !pyr || pyr->ctx != c) { hv_set_error("%s: invalid context / pyramid", who); return HV_ERR_INVALID; }
+    if (capacity < 0 || !count || (capacity > 0 && !xy)) { hv_set_error("%s: NULL buffer or negative capacity (%d)", who, capacity); return HV_ERR_INVALID; }
+    const HvLevel& L = pyr->desc.lv[0];
+    memset(&a, 0, sizeof(a));
+    a.gray = L.gray; a.pitch = L.gpitch; a.w = L.w; a.h = L.h;
+    a.threshold = threshold < 0 ? 0 : (threshold > 255 ? 255 : threshold);       // FAST_t: std::min(std::max(threshold, 0), 255)
+    a.nonmax = nonmax ? 1 : 0;
+    a.tilesX = (L.w + 31) / 32; a.tilesY = (L.h + 7) / 8;
+    a.xy = (float2*)xy; a.response = response; a.capacity = capacity; a.count = count;
+    *scratch = align_up(sizeof(unsigned) * 8 * (size_t)a.tilesX * a.tilesY + sizeof(int) * (size_t)a.tilesX * a.tilesY, 256);
+    return HV_OK;
+}
+
+// points the jobs' masks and tile counts into the context's FAST scratch, grown (after the work that may still read it) as needed
+static int fast_scratch(hv_ctx* c, FastArgs* jobs, const size_t* bytes, int njobs)
+{
+    size_t total = 0;
+    for (int j = 0; j < njobs; j++) total += bytes[j];
+    if (total > c->fastScratchBytes) {
+        if (c->d_fastScratch) { HV_CUDA(cudaStreamSynchronize(c->stream)); cudaFree(c->d_fastScratch); }
+        c->d_fastScratch = nullptr; c->fastScratchBytes = 0;
+        size_t cap = 65536; while (cap < total) cap *= 2;
+        HV_CUDA(cudaMalloc(&c->d_fastScratch, cap));
+        c->fastScratchBytes = cap;
+    }
+    uint8_t* p = (uint8_t*)c->d_fastScratch;
+    for (int j = 0; j < njobs; j++) {
+        FastArgs& a = jobs[j];
+        a.mask = (unsigned*)p;
+        a.tileCount = (int*)(p + sizeof(unsigned) * 8 * (size_t)a.tilesX * a.tilesY);
+        p += bytes[j];
+    }
+    return HV_OK;
+}
+
+int hv_fast_detect_device(hv_ctx* c, hv_pyr* pyr, int threshold, int nonmax, float* dXY, float* dResponse, int capacity, int* dCount)
+{
+    FastArgs a;
+    size_t bytes = 0;
+    int rc = fast_args("hv_fast_detect_device", c, pyr, threshold, nonmax, dXY, dResponse, capacity, dCount, a, &bytes);
+    if (rc != HV_OK) return rc;
+    HV_CUDA(cudaSetDevice(c->device));
+    rc = fast_scratch(c, &a, &bytes, 1);
+    if (rc != HV_OK) return rc;
+    HV_CUDA(hv_launch_fast(a, c->stream));
+    c->launches += 2;
+    return HV_OK;
+}
+
+int hv_fast_detect(hv_ctx* c, hv_pyr* pyr, int threshold, int nonmax, float* xy, float* response, int capacity, int* count)
+{
+    FastArgs a;
+    size_t bytes = 0;
+    int rc = fast_args("hv_fast_detect", c, pyr, threshold, nonmax, xy, response, capacity, count, a, &bytes);
+    if (rc != HV_OK) return rc;
+    HV_CUDA(cudaSetDevice(c->device));
+    rc = fast_scratch(c, &a, &bytes, 1);
+    if (rc != HV_OK) return rc;
+    // staging block: [count (16 bytes) | xy 8 capacity | response 4 capacity]
+    const size_t oXY = 16, oResp = oXY + 8 * (size_t)capacity, total = oResp + (response ? 4 * (size_t)capacity : 0);
+    rc = hv_ctx_reserve_stage(c, total);
+    if (rc != HV_OK) return rc;
+    uint8_t* hs = (uint8_t*)c->h_stage; uint8_t* ds = (uint8_t*)c->d_stage;
+    a.count = (int*)ds; a.xy = (float2*)(ds + oXY); a.response = response ? (float*)(ds + oResp) : nullptr;
+    HV_CUDA(hv_launch_fast(a, c->stream));
+    c->launches += 2;
+    HV_CUDA(cudaMemcpyAsync(hs, ds, total, cudaMemcpyDeviceToHost, c->stream));
+    HV_CUDA(cudaStreamSynchronize(c->stream));
+    memcpy(count, hs, sizeof(int));
+    if (capacity > 0) memcpy(xy, hs + oXY, 8 * (size_t)capacity);
+    if (response && capacity > 0) memcpy(response, hs + oResp, 4 * (size_t)capacity);
+    return HV_OK;
+}
+
+int hv_fast_detect_batch_device(hv_ctx* c, const hv_fast_job* jobs, int njobs, int threshold, int nonmax)
+{
+    int rc = corner_batch_check("hv_fast_detect_batch_device", c, jobs, njobs);
+    if (rc != HV_OK) return rc;
+    FastBatchArgs b;
+    memset(&b, 0, sizeof(b));
+    size_t bytes[HV_CORNER_BATCH_MAX];
+    long long tiles = 0, bands = 0;
+    for (int j = 0; j < njobs; j++) {
+        const hv_fast_job& J = jobs[j];
+        char who[64];
+        snprintf(who, sizeof(who), "hv_fast_detect_batch_device job %d", j);
+        rc = fast_args(who, c, J.pyr, threshold, nonmax, J.d_xy, J.d_response, J.capacity, J.d_count, b.job[j], &bytes[j]);
+        if (rc != HV_OK) return rc;
+        b.firstTile[j] = (int)tiles; b.firstBand[j] = (int)bands;
+        tiles += (long long)b.job[j].tilesX * b.job[j].tilesY;
+        bands += b.job[j].tilesY;
+        if (tiles > INT_MAX) { hv_set_error("%s: more than %d tiles in one batch", who, INT_MAX); return HV_ERR_INVALID; }
+    }
+    for (int j = njobs; j <= HV_CORNER_BATCH_MAX; j++) { b.firstTile[j] = (int)tiles; b.firstBand[j] = (int)bands; }
+    HV_CUDA(cudaSetDevice(c->device));
+    rc = fast_scratch(c, b.job, bytes, njobs);
+    if (rc != HV_OK) return rc;
+    HV_CUDA(hv_launch_fast_batch(b, njobs, c->stream));
+    c->launches += 2;
     return HV_OK;
 }
 

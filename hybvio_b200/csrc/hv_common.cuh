@@ -155,6 +155,28 @@ struct SubpixBatchArgs {
 static_assert(sizeof(SubpixBatchArgs) <= HV_KERNEL_PARAM_MAX, "sub-pixel batch arguments exceed the kernel-parameter space");
 cudaError_t hv_launch_subpix_batch(const SubpixBatchArgs& b, int njobs, cudaStream_t stream);
 
+// ---- FAST corner detection (fast.cu): cv::FAST, TYPE_9_16, on level 0
+struct FastArgs {
+    const uint8_t* gray; int pitch, w, h;
+    int threshold;                    // already clamped to [0, 255]
+    int nonmax;
+    int tilesX, tilesY;               // ceil(w / 32) x ceil(h / 8) tiles
+    unsigned* mask;                   // scratch: 8 tilesY x tilesX keypoint masks, row-major over (row, tile)
+    int* tileCount;                   // scratch: tilesY x tilesX keypoint counts
+    float2* xy; float* response;      // capacity slots each; response may be NULL
+    int capacity;
+    int* count;                       // the full count, which may exceed capacity
+};
+cudaError_t hv_launch_fast(const FastArgs& a, cudaStream_t stream);         // two launches: mark + count, then scan + scatter
+
+struct FastBatchArgs {
+    FastArgs job[HV_CORNER_BATCH_MAX];
+    int firstTile[HV_CORNER_BATCH_MAX + 1];   // first CTA (tile) of job j in the mark grid; firstTile[njobs ..] = that grid
+    int firstBand[HV_CORNER_BATCH_MAX + 1];   // first CTA (band of 8 rows) of job j in the scatter grid; firstBand[njobs ..] = that grid
+};
+static_assert(sizeof(FastBatchArgs) <= HV_KERNEL_PARAM_MAX, "FAST batch arguments exceed the kernel-parameter space");
+cudaError_t hv_launch_fast_batch(const FastBatchArgs& b, int njobs, cudaStream_t stream);
+
 // ---- frame ingest (ingest.cu)
 #define HV_REMAP_INVALID (-32768)
 struct HvRemapEntry { short x0, y0; float xfrac, yfrac; };      // 12 bytes per output pixel (hv_remap_entry of the C ABI)

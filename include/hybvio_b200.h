@@ -206,6 +206,31 @@ typedef struct hv_subpix_job { hv_pyr* pyr; float* d_xy; int n; } hv_subpix_job;
 int hv_subpix_refine_batch_device(hv_ctx* ctx, const hv_subpix_job* jobs, int njobs, int win_w, int win_h, int zero_w, int zero_h,
                                   int criteria_type, int max_count, double epsilon);
 
+/* ---------------------------------------------------------------- FAST corner detection ----------------------- */
+/* cv::FAST(level 0 of pyr, keypoints, threshold, nonmax, FastFeatureDetector::TYPE_9_16) (OCV/features2d/src/fast.cpp, fast_score.cpp):
+ * the detector the reference's FeatureDetector::build hands out for featureDetector = FAST (src/tracker/feature_detector_legacy.cpp;
+ * how that adapter post-processes the keypoints is not restated here), on the level-0 image that hv_pyr_build / hv_pyr_build_batch /
+ * hv_ingest_frame(s) has already put into HBM. threshold is clamped to [0, 255] as FAST_t clamps it; nonmax != 0 keeps a corner only when
+ * its score is strictly above its 8 neighbours'. Bit-identical to cv::FAST built without or with IPP for thresholds in [0, 255].
+ *   xy        capacity x (x, y) float32: the keypoints in OpenCV's order (rows top to bottom, columns left to right); slots
+ *             [count, capacity) are set to (HV_CORNER_NONE, HV_CORNER_NONE), so hv_subpix_refine_device and hv_lk_track_device can
+ *             run over `capacity` without the count reaching the host (as with hv_gftt_select_device)
+ *   response  capacity x float32 or NULL: the keypoint's score with suppression (cornerScore<16>), 0 without it (the KeyPoint
+ *             response cv::FAST reports); 0 in the slots [count, capacity)
+ *   count     the full count, which may exceed capacity: only the first `capacity` keypoints are written
+ * Errors, before anything is launched (buffers and the context's launch count untouched): HV_ERR_INVALID for a NULL context / pyramid /
+ * count, a NULL xy with capacity > 0, a pyramid of another context or a negative capacity.
+ * Every call is two launches (ctx's launch count + 2); an image smaller than 7 x 7 yields count 0. */
+int hv_fast_detect(hv_ctx* ctx, hv_pyr* pyr, int threshold, int nonmax, float* xy, float* response, int capacity, int* count);   /* host, synchronises */
+int hv_fast_detect_device(hv_ctx* ctx, hv_pyr* pyr, int threshold, int nonmax, float* d_xy, float* d_response, int capacity,
+                          int* d_count);                                                                             /* device, asynchronous */
+/* hv_fast_detect_device for up to HV_CORNER_BATCH_MAX pyramids (one per session sharing the context) in the two launches of one call:
+ * every job's outputs are bit-identical to the per-frame call's. Pyramids may differ in size and pitch; threshold and nonmax are the
+ * batch's. Errors as hv_fast_detect_device's for every job, and HV_ERR_INVALID for a NULL jobs array or njobs outside
+ * 1..HV_CORNER_BATCH_MAX, all before anything is launched. */
+typedef struct hv_fast_job { hv_pyr* pyr; float* d_xy; float* d_response; int capacity; int* d_count; } hv_fast_job;
+int hv_fast_detect_batch_device(hv_ctx* ctx, const hv_fast_job* jobs, int njobs, int threshold, int nonmax);
+
 /* ---------------------------------------------------------------- frame ingest (SURVEY.md 8(f) N4) -------- */
 /* Device part of tracker::Image::Factory::build / buildStereo (src/tracker/image.cpp:243-308): colour -> gray
  * (accelerated-arrays pixelwiseAffine, image.cpp:360-366) and undistortion / rectification (UndistorterImplementation::undistort,
