@@ -92,6 +92,13 @@ class FastJob(ctypes.Structure):
     _fields_ = [("pyr", c_void_p), ("d_xy", c_void_p), ("d_response", c_void_p), ("capacity", c_int), ("d_count", c_void_p)]
 
 
+class GoodFeaturesJob(ctypes.Structure):
+    """hv_good_features_job: one session's pyramid, corner budget, mask and outputs in the batched Shi-Tomasi detection (see
+    good_features_job)"""
+    _fields_ = [("pyr", c_void_p), ("max_corners", c_int), ("d_mask", c_void_p), ("mask_stride", c_size_t), ("d_xy", c_void_p),
+                ("d_response", c_void_p), ("capacity", c_int), ("d_count", c_void_p)]
+
+
 CORNER_BATCH_MAX = 64   # HV_CORNER_BATCH_MAX
 
 
@@ -154,6 +161,9 @@ def load():
     lib.hv_fast_detect.argtypes = [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p]
     lib.hv_fast_detect_device.argtypes = lib.hv_fast_detect.argtypes
     lib.hv_fast_detect_batch_device.argtypes = [c_void_p, ctypes.POINTER(FastJob), c_int, c_int, c_int]
+    lib.hv_good_features.argtypes = [c_void_p, c_void_p, c_int, c_int, c_double, c_double, c_void_p, c_size_t, c_void_p, c_void_p, c_int, c_void_p]
+    lib.hv_good_features_device.argtypes = lib.hv_good_features.argtypes
+    lib.hv_good_features_batch_device.argtypes = [c_void_p, ctypes.POINTER(GoodFeaturesJob), c_int, c_int, c_double, c_double]
     _bind_ekf(lib)
     _lib = lib
     return lib
@@ -375,6 +385,13 @@ class Context:
         J = (FastJob * len(jobs))(*jobs)
         check(self.lib.hv_fast_detect_batch_device(self.h, J, len(jobs), threshold, 1 if nonmax else 0), "hv_fast_detect_batch_device")
 
+    def good_features_batch_device(self, jobs, quality_level=0.01, min_distance=10.0, block_size=3):
+        """hv_good_features_batch_device: cv::goodFeaturesToTrack on level 0 of every job's pyramid (see good_features_job), three
+        launches; asynchronous."""
+        J = (GoodFeaturesJob * len(jobs))(*jobs)
+        check(self.lib.hv_good_features_batch_device(self.h, J, len(jobs), block_size, quality_level, min_distance),
+              "hv_good_features_batch_device")
+
     def lk_track_device(self, prev, nxt, d_prev, d_next, d_status, d_ts, n, use_initial, max_iter=20, eps=0.03, min_eig=1e-3):
         check(self.lib.hv_lk_track_device(self.h, prev.h, nxt.h, _ptr(d_prev), _ptr(d_next), _ptr(d_status), _ptr(d_ts), n,
                                           1 if use_initial else 0, max_iter, eps, min_eig), "hv_lk_track_device")
@@ -417,6 +434,28 @@ def fast_job(pyr, d_xy, d_count, d_response=None):
     for t in (d_xy, d_count) + (() if d_response is None else (d_response,)):
         _check_cuda_buffer(t)
     return FastJob(pyr.h.value, _ptr(d_xy), _ptr(d_response), d_xy.numel() // 2, _ptr(d_count))
+
+
+def _mask_tensor(d_mask, pyr):
+    """A CUDA uint8 mask of level 0's shape (h, w) whose rows are dense: (pointer, row stride in bytes); None: (None, 0)."""
+    if d_mask is None:
+        return None, 0
+    import torch
+    w, h = pyr.level_size(0)
+    if not d_mask.is_cuda or d_mask.dtype != torch.uint8 or d_mask.dim() != 2 or d_mask.stride(1) != 1:
+        raise ValueError("the mask must be a 2-D uint8 CUDA tensor with dense rows")
+    if tuple(d_mask.shape) != (h, w):
+        raise ValueError(f"the mask is {tuple(d_mask.shape)}, level 0 is {(h, w)}")
+    return d_mask.data_ptr(), d_mask.stride(0)
+
+
+def good_features_job(pyr, d_xy, d_count, max_corners, d_response=None, d_mask=None):
+    """A GoodFeaturesJob on CUDA tensors: d_xy (capacity, 2) float32, d_count (1,) int32, d_response (capacity,) float32 or None,
+    d_mask (h, w) uint8 with dense rows (any row stride) or None. The tensors must outlive the call that uses the job."""
+    for t in (d_xy, d_count) + (() if d_response is None else (d_response,)):
+        _check_cuda_buffer(t)
+    mp, ms = _mask_tensor(d_mask, pyr)
+    return GoodFeaturesJob(pyr.h.value, max_corners, mp, ms, _ptr(d_xy), _ptr(d_response), d_xy.numel() // 2, _ptr(d_count))
 
 
 def _dense_rows(img):
@@ -557,6 +596,35 @@ class Pyramid:
             _check_cuda_buffer(t)
         check(self.lib.hv_fast_detect_device(self.ctx.h, self.h, threshold, 1 if nonmax else 0, _ptr(d_xy), _ptr(d_response),
                                              d_xy.numel() // 2, _ptr(d_count)), "hv_fast_detect_device")
+
+    def good_features(self, max_corners, quality_level, min_distance, mask=None, block_size=3):
+        """cv::goodFeaturesToTrack (minimum-eigenvalue response) on the level-0 image of this pyramid. mask: None or an (h, w) uint8
+        array (non-zero: allowed). Returns (xy (n, 2) float32, response (n,) float32) in OpenCV's order, n <= max_corners."""
+        mp, ms = None, 0
+        if mask is not None:
+            mask = np.asarray(mask)
+            w, h = self.level_size(0)
+            if mask.shape != (h, w):
+                raise ValueError(f"the mask is {mask.shape}, level 0 is {(h, w)}")
+            if mask.dtype != np.uint8 or mask.strides[1] != 1 or mask.strides[0] < w:
+                mask = np.ascontiguousarray(mask, np.uint8)
+            mp, ms = mask.ctypes.data, mask.strides[0]
+        cap = max(int(max_corners), 1)
+        xy = np.zeros((cap, 2), np.float32)
+        resp = np.zeros(cap, np.float32)
+        n = c_int(0)
+        check(self.lib.hv_good_features(self.ctx.h, self.h, block_size, max_corners, quality_level, min_distance, mp, ms, _ptr(xy),
+                                        _ptr(resp), cap, ctypes.byref(n)), "hv_good_features")
+        return xy[:n.value].copy(), resp[:n.value].copy()
+
+    def good_features_device(self, d_xy, d_count, max_corners, quality_level, min_distance, d_response=None, d_mask=None, block_size=3):
+        """hv_good_features_device on CUDA tensors: d_xy (capacity, 2) float32, d_count (1,) int32, d_response (capacity,) float32 or
+        None, d_mask (h, w) uint8 with dense rows or None; asynchronous on the context's stream."""
+        for t in (d_xy, d_count) + (() if d_response is None else (d_response,)):
+            _check_cuda_buffer(t)
+        mp, ms = _mask_tensor(d_mask, self)
+        check(self.lib.hv_good_features_device(self.ctx.h, self.h, block_size, max_corners, quality_level, min_distance, mp, ms,
+                                               _ptr(d_xy), _ptr(d_response), d_xy.numel() // 2, _ptr(d_count)), "hv_good_features_device")
 
     def release(self):
         if self.h:

@@ -78,6 +78,7 @@ int hv_ctx_destroy(hv_ctx* c)
     if (c->d_done) cudaFree(c->d_done);
     if (c->d_selectScratch) cudaFree(c->d_selectScratch);
     if (c->d_fastScratch) cudaFree(c->d_fastScratch);
+    if (c->d_gfScratch) cudaFree(c->d_gfScratch);
     if (c->d_ekfStage) cudaFree(c->d_ekfStage);
     for (int i = 0; i < HV_EKF_STAGES; i++) {
         if (c->h_ekfStage[i]) cudaFreeHost(c->h_ekfStage[i]);
@@ -916,6 +917,166 @@ int hv_fast_detect_batch_device(hv_ctx* c, const hv_fast_job* jobs, int njobs, i
     if (rc != HV_OK) return rc;
     HV_CUDA(hv_launch_fast_batch(b, njobs, c->stream));
     c->launches += 2;
+    return HV_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ Shi-Tomasi corner detection (N2)
+// Scratch: HV_CORNER_BATCH_MAX (max word, candidate count) pairs at the front (job j of a call uses pair j; the call zeroes the pairs it
+// uses on the stream before its first launch), then per job its response map, candidate keys and min-distance grid.
+static const size_t GF_WORDS = align_up(HV_CORNER_BATCH_MAX * 2 * sizeof(unsigned), 256);
+
+// Checks one job and fills everything but the scratch; *scratch = the bytes of map, keys and grid it needs.
+static int gf_args(const char* who, hv_ctx* c, hv_pyr* pyr, int blockSize, int maxCorners, double quality, double minDistance,
+                   const uint8_t* mask, size_t maskStride, float* xy, float* response, int capacity, int* count, GoodFeaturesArgs& a,
+                   size_t* scratch)
+{
+    if (!c || !pyr || pyr->ctx != c) { hv_set_error("%s: invalid context / pyramid", who); return HV_ERR_INVALID; }
+    if (!xy || !count) { hv_set_error("%s: NULL xy or count", who); return HV_ERR_INVALID; }
+    if (blockSize != 3) { hv_set_error("%s: block size %d unsupported (3 only)", who, blockSize); return HV_ERR_UNSUPPORTED; }
+    if (maxCorners < 1) { hv_set_error("%s: max_corners %d unsupported (1 or more)", who, maxCorners); return HV_ERR_UNSUPPORTED; }
+    if (capacity < maxCorners) { hv_set_error("%s: capacity %d below max_corners %d", who, capacity, maxCorners); return HV_ERR_INVALID; }
+    if (!(quality > 0.0)) { hv_set_error("%s: quality_level %g (must be > 0)", who, quality); return HV_ERR_INVALID; }
+    if (!(minDistance >= 0.0) || !std::isfinite(minDistance)) {
+        hv_set_error("%s: min_distance %g (must be finite and >= 0)", who, minDistance);
+        return HV_ERR_INVALID;
+    }
+    const HvLevel& L = pyr->desc.lv[0];
+    if (mask && maskStride < (size_t)L.w) { hv_set_error("%s: mask stride %zu below the width %d", who, maskStride, L.w); return HV_ERR_INVALID; }
+    if (mask && maskStride > (size_t)INT_MAX) { hv_set_error("%s: mask stride %zu too large", who, maskStride); return HV_ERR_INVALID; }
+    memset(&a, 0, sizeof(a));
+    a.gray = L.gray; a.pitch = L.gpitch; a.w = L.w; a.h = L.h;
+    a.mask = mask; a.maskPitch = (int)maskStride;
+    a.tilesX = (L.w + 31) / 32; a.tilesY = (L.h + 7) / 8;
+    a.maxCorners = maxCorners; a.quality = quality;
+    a.xy = (float2*)xy; a.response = response; a.capacity = capacity; a.count = count;
+    a.useGrid = minDistance >= 1.0;
+    size_t gridBytes = 0;
+    if (a.useGrid) {
+        // cell side s: the largest with 2 (s - 1)^2 < minDistance^2, so two corners in one cell are always too close and a cell holds at
+        // most one kept corner; s - 1 <= 2896 keeps (s - 1)^2 exact in the fp32 distance test. reach: the largest |dx| that can be too close.
+        const int big = L.w > L.h ? L.w : L.h;
+        a.md2 = minDistance * minDistance;
+        long long s = (long long)(minDistance / 1.4142135623730951);
+        if (s > 2897) s = 2897;
+        if (s < 1) s = 1;
+        while (s > 1 && 2.0 * (double)(s - 1) * (double)(s - 1) >= a.md2) s--;
+        while (s < 2897 && 2.0 * (double)s * (double)s < a.md2) s++;
+        a.cell = (int)s;
+        const double r = std::ceil(minDistance) - 1.0;
+        a.reach = r > (double)big ? big : (int)r;
+        a.gridW = (L.w + a.cell - 1) / a.cell; a.gridH = (L.h + a.cell - 1) / a.cell;
+        gridBytes = align_up(sizeof(int) * (size_t)a.gridW * a.gridH, 256);
+    }
+    const size_t interior = L.w > 2 && L.h > 2 ? (size_t)(L.w - 2) * (L.h - 2) : 1;
+    *scratch = align_up(sizeof(float) * (size_t)L.w * L.h, 256) + align_up(sizeof(unsigned long long) * interior, 256) + gridBytes;
+    return HV_OK;
+}
+
+// points the jobs' words, maps, keys and grids into the context's scratch, grown (after the work that may still read it) as needed
+static int gf_scratch(hv_ctx* c, GoodFeaturesArgs* jobs, const size_t* bytes, int njobs)
+{
+    size_t total = GF_WORDS;
+    for (int j = 0; j < njobs; j++) total += bytes[j];
+    if (total > c->gfScratchBytes) {
+        if (c->d_gfScratch) { HV_CUDA(cudaStreamSynchronize(c->stream)); cudaFree(c->d_gfScratch); }
+        c->d_gfScratch = nullptr; c->gfScratchBytes = 0;
+        size_t cap = 1 << 20; while (cap < total) cap *= 2;
+        HV_CUDA(cudaMalloc(&c->d_gfScratch, cap));
+        c->gfScratchBytes = cap;
+    }
+    HV_CUDA(cudaMemsetAsync(c->d_gfScratch, 0, 2 * sizeof(unsigned) * (size_t)njobs, c->stream));
+    uint8_t* p = (uint8_t*)c->d_gfScratch;
+    unsigned* words = (unsigned*)p;
+    p += GF_WORDS;
+    for (int j = 0; j < njobs; j++) {
+        GoodFeaturesArgs& a = jobs[j];
+        a.maxWord = words + 2 * j;
+        a.nCand = (int*)(words + 2 * j + 1);
+        uint8_t* q = p;
+        a.eig = (float*)q; q += align_up(sizeof(float) * (size_t)a.w * a.h, 256);
+        a.maxCand = a.w > 2 && a.h > 2 ? (a.w - 2) * (a.h - 2) : 1;
+        a.keys = (unsigned long long*)q; q += align_up(sizeof(unsigned long long) * (size_t)a.maxCand, 256);
+        a.grid = a.useGrid ? (int*)q : nullptr;
+        p += bytes[j];
+    }
+    return HV_OK;
+}
+
+int hv_good_features_device(hv_ctx* c, hv_pyr* pyr, int blockSize, int maxCorners, double quality, double minDistance,
+                            const uint8_t* dMask, size_t maskStride, float* dXY, float* dResponse, int capacity, int* dCount)
+{
+    GoodFeaturesArgs a;
+    size_t bytes = 0;
+    int rc = gf_args("hv_good_features_device", c, pyr, blockSize, maxCorners, quality, minDistance, dMask, maskStride, dXY, dResponse,
+                     capacity, dCount, a, &bytes);
+    if (rc != HV_OK) return rc;
+    HV_CUDA(cudaSetDevice(c->device));
+    rc = gf_scratch(c, &a, &bytes, 1);
+    if (rc != HV_OK) return rc;
+    HV_CUDA(hv_launch_good_features(a, c->stream));
+    c->launches += 3;
+    return HV_OK;
+}
+
+int hv_good_features(hv_ctx* c, hv_pyr* pyr, int blockSize, int maxCorners, double quality, double minDistance, const uint8_t* mask,
+                     size_t maskStride, float* xy, float* response, int capacity, int* count)
+{
+    GoodFeaturesArgs a;
+    size_t bytes = 0;
+    int rc = gf_args("hv_good_features", c, pyr, blockSize, maxCorners, quality, minDistance, mask, maskStride, xy, response, capacity,
+                     count, a, &bytes);
+    if (rc != HV_OK) return rc;
+    HV_CUDA(cudaSetDevice(c->device));
+    rc = gf_scratch(c, &a, &bytes, 1);
+    if (rc != HV_OK) return rc;
+    // staging block: [count (16 bytes) | xy 8 capacity | response 4 capacity | mask]
+    const size_t oXY = 16, oResp = oXY + 8 * (size_t)capacity, oMask = align_up(oResp + (response ? 4 * (size_t)capacity : 0), 16);
+    const size_t maskBytes = mask ? maskStride * (size_t)(a.h - 1) + (size_t)a.w : 0;
+    rc = hv_ctx_reserve_stage(c, oMask + maskBytes);
+    if (rc != HV_OK) return rc;
+    uint8_t* hs = (uint8_t*)c->h_stage; uint8_t* ds = (uint8_t*)c->d_stage;
+    if (mask) {
+        memcpy(hs + oMask, mask, maskBytes);
+        HV_CUDA(cudaMemcpyAsync(ds + oMask, hs + oMask, maskBytes, cudaMemcpyHostToDevice, c->stream));
+        a.mask = ds + oMask;
+    }
+    a.count = (int*)ds; a.xy = (float2*)(ds + oXY); a.response = response ? (float*)(ds + oResp) : nullptr;
+    HV_CUDA(hv_launch_good_features(a, c->stream));
+    c->launches += 3;
+    HV_CUDA(cudaMemcpyAsync(hs, ds, oMask, cudaMemcpyDeviceToHost, c->stream));
+    HV_CUDA(cudaStreamSynchronize(c->stream));
+    memcpy(count, hs, sizeof(int));
+    memcpy(xy, hs + oXY, 8 * (size_t)capacity);
+    if (response) memcpy(response, hs + oResp, 4 * (size_t)capacity);
+    return HV_OK;
+}
+
+int hv_good_features_batch_device(hv_ctx* c, const hv_good_features_job* jobs, int njobs, int blockSize, double quality, double minDistance)
+{
+    int rc = corner_batch_check("hv_good_features_batch_device", c, jobs, njobs);
+    if (rc != HV_OK) return rc;
+    GoodFeaturesBatchArgs b;
+    memset(&b, 0, sizeof(b));
+    size_t bytes[HV_CORNER_BATCH_MAX];
+    long long tiles = 0, strips = 0;
+    for (int j = 0; j < njobs; j++) {
+        const hv_good_features_job& J = jobs[j];
+        char who[64];
+        snprintf(who, sizeof(who), "hv_good_features_batch_device job %d", j);
+        rc = gf_args(who, c, J.pyr, blockSize, J.max_corners, quality, minDistance, J.d_mask, J.mask_stride, J.d_xy, J.d_response,
+                     J.capacity, J.d_count, b.job[j], &bytes[j]);
+        if (rc != HV_OK) return rc;
+        b.firstTile[j] = (int)tiles; b.firstStrip[j] = (int)strips;
+        tiles += (long long)b.job[j].tilesX * b.job[j].tilesY;
+        strips += (b.job[j].w + 31) / 32;
+        if (tiles > INT_MAX) { hv_set_error("%s: more than %d tiles in one batch", who, INT_MAX); return HV_ERR_INVALID; }
+    }
+    for (int j = njobs; j <= HV_CORNER_BATCH_MAX; j++) { b.firstTile[j] = (int)tiles; b.firstStrip[j] = (int)strips; }
+    HV_CUDA(cudaSetDevice(c->device));
+    rc = gf_scratch(c, b.job, bytes, njobs);
+    if (rc != HV_OK) return rc;
+    HV_CUDA(hv_launch_good_features_batch(b, njobs, c->stream));
+    c->launches += 3;
     return HV_OK;
 }
 

@@ -177,6 +177,39 @@ struct FastBatchArgs {
 static_assert(sizeof(FastBatchArgs) <= HV_KERNEL_PARAM_MAX, "FAST batch arguments exceed the kernel-parameter space");
 cudaError_t hv_launch_fast_batch(const FastBatchArgs& b, int njobs, cudaStream_t stream);
 
+// ---- Shi-Tomasi corner detection (good_features.cu): cv::goodFeaturesToTrack with the minimum-eigenvalue response, block size 3
+#ifndef HV_GF_CHUNK                   // (a power of two; the emulator test builds with a small one to run many rounds on small images)
+#define HV_GF_CHUNK 8192              // sorted keys per selection round: 64 KB of dynamic shared memory
+#endif
+struct GoodFeaturesArgs {
+    const uint8_t* gray; int pitch, w, h;
+    const uint8_t* mask; int maskPitch;   // NULL: no mask
+    int tilesX, tilesY;               // ceil(w / 32) x ceil(h / 8) tiles
+    int maxCorners;
+    double quality;                   // qualityLevel
+    double md2;                       // minDistance^2
+    int useGrid;                      // minDistance >= 1: the greedy distance filter
+    int cell, reach, gridW, gridH;    // its grid: cell side (at most one kept corner per cell), +-reach pixels searched, cells per axis
+    float* eig;                       // scratch: w x h response map
+    unsigned long long* keys;         // scratch: maxCand = max(1, (w - 2)(h - 2)) candidate keys
+    int maxCand;
+    int* grid;                        // scratch: gridW x gridH, the pixel index of the cell's kept corner or -1
+    unsigned* maxWord;                // scratch: the masked maximum as order-preserving bits, 0: no pixel
+    int* nCand;                       // scratch: the candidate count (maxWord and nCand are zeroed before the first launch)
+    float2* xy; float* response;      // capacity slots each; response may be NULL
+    int capacity;
+    int* count;
+};
+cudaError_t hv_launch_good_features(const GoodFeaturesArgs& a, cudaStream_t stream);     // three launches: response, candidates, select
+
+struct GoodFeaturesBatchArgs {
+    GoodFeaturesArgs job[HV_CORNER_BATCH_MAX];
+    int firstStrip[HV_CORNER_BATCH_MAX + 1];  // first CTA (32 columns) of job j in the response grid; firstStrip[njobs ..] = that grid
+    int firstTile[HV_CORNER_BATCH_MAX + 1];   // first CTA (tile) of job j in the candidate grid; firstTile[njobs ..] = that grid
+};
+static_assert(sizeof(GoodFeaturesBatchArgs) <= HV_KERNEL_PARAM_MAX, "good-features batch arguments exceed the kernel-parameter space");
+cudaError_t hv_launch_good_features_batch(const GoodFeaturesBatchArgs& b, int njobs, cudaStream_t stream);
+
 // ---- frame ingest (ingest.cu)
 #define HV_REMAP_INVALID (-32768)
 struct HvRemapEntry { short x0, y0; float xfrac, yfrac; };      // 12 bytes per output pixel (hv_remap_entry of the C ABI)

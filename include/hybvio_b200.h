@@ -231,6 +231,45 @@ int hv_fast_detect_device(hv_ctx* ctx, hv_pyr* pyr, int threshold, int nonmax, f
 typedef struct hv_fast_job { hv_pyr* pyr; float* d_xy; float* d_response; int capacity; int* d_count; } hv_fast_job;
 int hv_fast_detect_batch_device(hv_ctx* ctx, const hv_fast_job* jobs, int njobs, int threshold, int nonmax);
 
+/* ---------------------------------------------------------------- Shi-Tomasi corner detection ----------------- */
+/* cv::goodFeaturesToTrack(level 0 of pyr, corners, max_corners, quality_level, min_distance, mask, cornersQuality, block_size = 3,
+ * gradientSize = 3, useHarrisDetector = false) (OCV/imgproc/src/featureselect.cpp, the CPU path): the primitive of the reference's
+ * featureDetector = GFTT setting (how its legacy detector post-processes the list is not restated here), on the level-0 image that
+ * hv_pyr_build / hv_pyr_build_batch / hv_ingest_frame(s) has already put into HBM. Not GPU-GFTT's response (hv_gftt_*): this one is
+ * cv::cornerMinEigenVal's, bit for bit. In order: the minimum-eigenvalue response; maxVal = its maximum over the mask's non-zero pixels
+ * (0 when the mask selects none); the response kept where it is > (float)(maxVal * quality_level); the candidates are the pixels of
+ * [1, w - 1) x [1, h - 1) under the mask whose kept response is non-zero and the maximum of its 3 x 3 neighbourhood; they are listed by
+ * response, descending, ties by descending pixel address (y w + x); with min_distance >= 1 a candidate is dropped when a corner kept
+ * before it lies at (float)dx^2 + (float)dy^2 < min_distance^2; the list stops at max_corners. Bit-identical to cv::goodFeaturesToTrack
+ * built without IPP and run on its baseline code path (cv::setUseOptimized(false)); DESIGN.md 4.10 says what the other paths change.
+ *   mask      NULL or w x h u8 with row stride mask_stride bytes (host memory for hv_good_features, device memory otherwise)
+ *   xy        capacity x (x, y) float32, integer-valued: the list; slots [count, capacity) are set to (HV_CORNER_NONE, HV_CORNER_NONE), so
+ *             hv_subpix_refine_device and hv_lk_track_device can run over `capacity` without the count reaching the host
+ *   response  capacity x float32 or NULL: the corner's response (OpenCV's cornersQuality); 0 in the slots [count, capacity)
+ *   count     the list's length, at most max_corners
+ * Errors, before anything is launched (buffers and the context's launch count untouched): HV_ERR_INVALID for a NULL context / pyramid /
+ * xy / count, a pyramid of another context, capacity < max_corners, quality_level <= 0 or NaN, min_distance < 0 or not finite, or a mask stride
+ * below the width; HV_ERR_UNSUPPORTED for block_size other than 3 or max_corners < 1 (OpenCV's "no limit").
+ * Every call is three launches (ctx's launch count + 3) whatever the image holds; an image smaller than 3 x 3 yields count 0. The
+ * response map, the candidate keys (8 bytes per interior pixel) and the min-distance grid live in scratch memory of the context, which
+ * only grows. */
+int hv_good_features(hv_ctx* ctx, hv_pyr* pyr, int block_size, int max_corners, double quality_level, double min_distance,
+                     const uint8_t* mask, size_t mask_stride, float* xy, float* response, int capacity, int* count);      /* host, synchronises */
+int hv_good_features_device(hv_ctx* ctx, hv_pyr* pyr, int block_size, int max_corners, double quality_level, double min_distance,
+                            const uint8_t* d_mask, size_t mask_stride, float* d_xy, float* d_response, int capacity, int* d_count);
+/* hv_good_features_device for up to HV_CORNER_BATCH_MAX pyramids (one per session sharing the context) in the three launches of one
+ * call: every job's outputs are bit-identical to the per-frame call's. Pyramids may differ in size and pitch; max_corners, the mask and
+ * the outputs are per job, block_size, quality_level and min_distance the batch's. Errors as hv_good_features_device's for every job,
+ * and HV_ERR_INVALID for a NULL jobs array or njobs outside 1..HV_CORNER_BATCH_MAX, all before anything is launched. */
+typedef struct hv_good_features_job {
+    hv_pyr* pyr; int max_corners;
+    const uint8_t* d_mask; size_t mask_stride;
+    float* d_xy; float* d_response; int capacity;
+    int* d_count;
+} hv_good_features_job;
+int hv_good_features_batch_device(hv_ctx* ctx, const hv_good_features_job* jobs, int njobs, int block_size, double quality_level,
+                                  double min_distance);
+
 /* ---------------------------------------------------------------- frame ingest (SURVEY.md 8(f) N4) -------- */
 /* Device part of tracker::Image::Factory::build / buildStereo (src/tracker/image.cpp:243-308): colour -> gray
  * (accelerated-arrays pixelwiseAffine, image.cpp:360-366) and undistortion / rectification (UndistorterImplementation::undistort,
