@@ -120,23 +120,22 @@ int hv_ctx_reserve_stage(hv_ctx* c, size_t bytes)
     return HV_OK;
 }
 
-// HV_NO_POLL=1: results come back with a D2H copy + stream synchronisation instead (A/B switch)
-bool hv_polling_enabled() { static const bool on = getenv("HV_NO_POLL") == nullptr; return on; }
-
-int hv_poll_flag(volatile unsigned* flag, unsigned seq, cudaStream_t stream, const char* who)
+// Arms the completion signal of a host-buffer launch of `units` CTAs on the context's stage; the flag sits right behind the stage.
+static HvDoneSignal done_arm(hv_ctx* c, unsigned units)
 {
-    for (unsigned long long spins = 1;; spins++) {
-        if (*flag == seq) break;
-        if ((spins & 0xfff) == 0) {
-            const cudaError_t q = cudaStreamQuery(stream);
-            if (q == cudaErrorNotReady) continue;
-            if (q != cudaSuccess) { hv_set_error("%s: %s while waiting for the result", who, cudaGetErrorString(q)); return HV_ERR_CUDA; }
-            if (*flag == seq) break;
-            hv_set_error("%s: the kernel finished without raising its completion flag", who); return HV_ERR_STATE;
-        }
+    c->doneCount += units;
+    return HvDoneSignal{c->d_done, c->doneCount, ++c->seq, (volatile unsigned*)((uint8_t*)c->hd_stage + c->stageBytes)};
+}
+
+// Waits for the flag of a signal from done_arm; on failure resynchronises the counter before anybody polls again.
+static int done_wait(hv_ctx* c, const HvDoneSignal& d, const char* who)
+{
+    volatile unsigned* flag = (volatile unsigned*)((uint8_t*)c->h_stage + c->stageBytes);
+    const int rc = hv_poll(c->stream, who, [&] { return *flag == d.seq; });
+    if (rc != HV_OK) {
+        cudaStreamSynchronize(c->stream); cudaMemsetAsync(c->d_done, 0, sizeof(unsigned), c->stream); cudaStreamSynchronize(c->stream); c->doneCount = 0;
     }
-    __atomic_thread_fence(__ATOMIC_ACQUIRE);
-    return HV_OK;
+    return rc;
 }
 
 // ------------------------------------------------------------------------------------------------ pyramid
@@ -306,7 +305,7 @@ static int lk_fill(LkLaunch& L, hv_ctx* c, int maxLevel, int maxIter, double eps
     double e = eps < 0. ? 0. : (eps > 10. ? 10. : eps);
     L.eps2 = e * e;
     L.minEig = (float)minEig;
-    L.doneCounter = nullptr; L.doneTarget = 0; L.seq = 0; L.hostFlag = nullptr;
+    L.done = HvDoneSignal{};
     return HV_OK;
 }
 
@@ -391,7 +390,7 @@ int hv_lk_track(hv_ctx* c, hv_pyr* prev, hv_pyr* next, const float* prevXY, floa
     uint8_t* hs = (uint8_t*)c->h_stage; uint8_t* ds = (uint8_t*)c->d_stage;
     memcpy(hs + oPrev, prevXY, 8 * (size_t)n);
     if (useInitial) memcpy(hs + oNext, nextXY, 8 * (size_t)n);
-    if (hv_polling_enabled() && hv_lk_uses_cta_kernel(n)) {     // only the CTA-per-feature kernel raises the host flag
+    if (hv_lk_uses_cta_kernel(n)) {     // only the CTA-per-feature kernel raises the host flag
         // The kernel reads the points from and writes the results to the mapped pinned block itself (a few KB over PCIe) and
         // raises a flag there when the last feature is done: no H2D / D2H copy calls, no stream synchronisation.
         uint8_t* hd = (uint8_t*)c->hd_stage;
@@ -402,18 +401,13 @@ int hv_lk_track(hv_ctx* c, hv_pyr* prev, hv_pyr* next, const float* prevXY, floa
         d.status = hd + oSt; d.trackStatus = (int32_t*)(hd + oTs); d.initPts = nullptr;
         L.njobs = 1;
         lk_fill(L, c, HV_MAX_LEVELS, maxIter, eps, minEig);
-        volatile unsigned* flag = (volatile unsigned*)(hs + c->stageBytes);
-        L.doneCounter = c->d_done; c->doneCount += (unsigned)n; L.doneTarget = c->doneCount;
-        L.seq = ++c->seq; L.hostFlag = (volatile unsigned*)(hd + c->stageBytes);
+        L.done = done_arm(c, (unsigned)n);
         cudaError_t e = hv_launch_lk(L, prev->win, c->stream);
         if (e == cudaErrorInvalidValue) { hv_set_error("hv_lk_track: window size %d unsupported (supported: 11, 15, 21, 31)", prev->win); return HV_ERR_UNSUPPORTED; }
         HV_CUDA(e);
         c->launches += 1;
-        rc = hv_poll_flag(flag, L.seq, c->stream, "hv_lk_track");
-        if (rc != HV_OK) {      // resynchronise the counter before anybody polls again
-            cudaStreamSynchronize(c->stream); cudaMemsetAsync(c->d_done, 0, sizeof(unsigned), c->stream); cudaStreamSynchronize(c->stream); c->doneCount = 0;
-            return rc;
-        }
+        rc = done_wait(c, L.done, "hv_lk_track");
+        if (rc != HV_OK) return rc;
     } else {
         HV_CUDA(cudaMemcpyAsync(ds, hs, useInitial ? 16 * (size_t)n : 8 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
         rc = hv_lk_track_device(c, prev, next, (const float*)(ds + oPrev), (float*)(ds + oNext), ds + oSt, (int32_t*)(ds + oTs),
@@ -475,28 +469,14 @@ int hv_gftt_detect(hv_ctx* c, hv_pyr* pyr, int blockSize, int cell, float minRes
     const size_t bytes = (size_t)cells * 3 * sizeof(float);
     rc = hv_ctx_reserve_stage(c, bytes);
     if (rc != HV_OK) return rc;
-    uint8_t* hs = (uint8_t*)c->h_stage;
-    if (hv_polling_enabled()) {
-        // the kernel writes the key points straight into the mapped pinned block and the last cell raises the flag (as the LK kernel does)
-        a.kp = (float*)c->hd_stage;
-        volatile unsigned* flag = (volatile unsigned*)(hs + c->stageBytes);
-        a.doneCounter = c->d_done; c->doneCount += (unsigned)cells; a.doneTarget = c->doneCount;
-        a.seq = ++c->seq; a.hostFlag = (volatile unsigned*)((uint8_t*)c->hd_stage + c->stageBytes);
-        HV_CUDA(hv_launch_gftt(a, c->stream));
-        c->launches += 1;
-        rc = hv_poll_flag(flag, a.seq, c->stream, "hv_gftt_detect");
-        if (rc != HV_OK) {
-            cudaStreamSynchronize(c->stream); cudaMemsetAsync(c->d_done, 0, sizeof(unsigned), c->stream); cudaStreamSynchronize(c->stream); c->doneCount = 0;
-            return rc;
-        }
-    } else {
-        a.kp = (float*)c->d_stage;
-        HV_CUDA(hv_launch_gftt(a, c->stream));
-        c->launches += 1;
-        HV_CUDA(cudaMemcpyAsync(hs, c->d_stage, bytes, cudaMemcpyDeviceToHost, c->stream));
-        HV_CUDA(cudaStreamSynchronize(c->stream));
-    }
-    memcpy(kp, hs, bytes);
+    // the kernel writes the key points straight into the mapped pinned block and the last cell raises the flag (as the LK kernel does)
+    a.kp = (float*)c->hd_stage;
+    a.done = done_arm(c, (unsigned)cells);
+    HV_CUDA(hv_launch_gftt(a, c->stream));
+    c->launches += 1;
+    rc = done_wait(c, a.done, "hv_gftt_detect");
+    if (rc != HV_OK) return rc;
+    memcpy(kp, c->h_stage, bytes);
     return HV_OK;
 }
 
@@ -573,7 +553,7 @@ int hv_gftt_corners(hv_ctx* c, hv_pyr* pyr, int blockSize, int cell, float minRe
         const size_t oCount = (8 * (size_t)nprev + 15) / 16 * 16, oCorners = oCount + 16, total = oCorners + 8 * (size_t)need;
         rc = hv_ctx_reserve_stage(c, total);
         if (rc != HV_OK) return rc;
-        uint8_t* hs = (uint8_t*)c->h_stage; uint8_t* ds = (uint8_t*)c->d_stage;
+        uint8_t* hs = (uint8_t*)c->h_stage; uint8_t* hd = (uint8_t*)c->hd_stage;
         float* dKp = c->d_selectScratch;
         if (nprev > 0) {
             memcpy(hs, prevXY, 8 * (size_t)nprev);
@@ -583,27 +563,13 @@ int hv_gftt_corners(hv_ctx* c, hv_pyr* pyr, int blockSize, int cell, float minRe
         HV_CUDA(hv_launch_gftt(g, c->stream));
         c->launches += 1;
         a.kp = dKp; a.prev = dKp + 3 * (size_t)nkp; a.capacity = need;
-        if (hv_polling_enabled()) {
-            // the select kernel writes the corners and the count straight into the mapped pinned block and raises the flag
-            uint8_t* hd = (uint8_t*)c->hd_stage;
-            a.out = (float*)(hd + oCorners); a.count = (int*)(hd + oCount);
-            volatile unsigned* flag = (volatile unsigned*)(hs + c->stageBytes);
-            a.doneCounter = c->d_done; c->doneCount += 1u; a.doneTarget = c->doneCount;
-            a.seq = ++c->seq; a.hostFlag = (volatile unsigned*)(hd + c->stageBytes);
-            HV_CUDA(hv_launch_gftt_select(a, c->stream));
-            c->launches += 1;
-            rc = hv_poll_flag(flag, a.seq, c->stream, "hv_gftt_corners");
-            if (rc != HV_OK) {
-                cudaStreamSynchronize(c->stream); cudaMemsetAsync(c->d_done, 0, sizeof(unsigned), c->stream); cudaStreamSynchronize(c->stream); c->doneCount = 0;
-                return rc;
-            }
-        } else {
-            a.out = (float*)(ds + oCorners); a.count = (int*)(ds + oCount);
-            HV_CUDA(hv_launch_gftt_select(a, c->stream));
-            c->launches += 1;
-            HV_CUDA(cudaMemcpyAsync(hs + oCount, ds + oCount, total - oCount, cudaMemcpyDeviceToHost, c->stream));
-            HV_CUDA(cudaStreamSynchronize(c->stream));
-        }
+        // the select kernel writes the corners and the count straight into the mapped pinned block and raises the flag
+        a.out = (float*)(hd + oCorners); a.count = (int*)(hd + oCount);
+        a.done = done_arm(c, 1u);
+        HV_CUDA(hv_launch_gftt_select(a, c->stream));
+        c->launches += 1;
+        rc = done_wait(c, a.done, "hv_gftt_corners");
+        if (rc != HV_OK) return rc;
         memcpy(&got, hs + oCount, sizeof(int));
         memcpy(corners, hs + oCorners, 8 * (size_t)got);
     }
@@ -689,30 +655,15 @@ int hv_subpix_refine(hv_ctx* c, hv_pyr* pyr, float* xy, int n, int hw, int hh, i
     const size_t bytes = (size_t)n * 2 * sizeof(float);
     rc = hv_ctx_reserve_stage(c, bytes);
     if (rc != HV_OK) return rc;
-    uint8_t* hs = (uint8_t*)c->h_stage;
-    memcpy(hs, xy, bytes);
-    if (hv_polling_enabled()) {
-        // the kernel refines the points in the mapped pinned block itself and the last corner raises the flag (as the LK kernel does)
-        a.xy = (float2*)c->hd_stage;
-        volatile unsigned* flag = (volatile unsigned*)(hs + c->stageBytes);
-        a.doneCounter = c->d_done; c->doneCount += (unsigned)n; a.doneTarget = c->doneCount;
-        a.seq = ++c->seq; a.hostFlag = (volatile unsigned*)((uint8_t*)c->hd_stage + c->stageBytes);
-        HV_CUDA(hv_launch_subpix(a, c->stream));
-        c->launches += 1;
-        rc = hv_poll_flag(flag, a.seq, c->stream, "hv_subpix_refine");
-        if (rc != HV_OK) {
-            cudaStreamSynchronize(c->stream); cudaMemsetAsync(c->d_done, 0, sizeof(unsigned), c->stream); cudaStreamSynchronize(c->stream); c->doneCount = 0;
-            return rc;
-        }
-    } else {
-        a.xy = (float2*)c->d_stage;
-        HV_CUDA(cudaMemcpyAsync(c->d_stage, hs, bytes, cudaMemcpyHostToDevice, c->stream));
-        HV_CUDA(hv_launch_subpix(a, c->stream));
-        c->launches += 1;
-        HV_CUDA(cudaMemcpyAsync(hs, c->d_stage, bytes, cudaMemcpyDeviceToHost, c->stream));
-        HV_CUDA(cudaStreamSynchronize(c->stream));
-    }
-    memcpy(xy, hs, bytes);
+    memcpy(c->h_stage, xy, bytes);
+    // the kernel refines the points in the mapped pinned block itself and the last corner raises the flag (as the LK kernel does)
+    a.xy = (float2*)c->hd_stage;
+    a.done = done_arm(c, (unsigned)n);
+    HV_CUDA(hv_launch_subpix(a, c->stream));
+    c->launches += 1;
+    rc = done_wait(c, a.done, "hv_subpix_refine");
+    if (rc != HV_OK) return rc;
+    memcpy(xy, c->h_stage, bytes);
     return HV_OK;
 }
 

@@ -54,9 +54,23 @@ struct hv_pyr {
 };
 
 int hv_ctx_reserve_stage(hv_ctx* ctx, size_t bytes);
-// Spins until *flag == seq (mapped pinned memory written by a kernel on `stream`); checks the stream for errors while waiting.
-int hv_poll_flag(volatile unsigned* flag, unsigned seq, cudaStream_t stream, const char* who);
-bool hv_polling_enabled();
+// Spins until done() holds (a condition on mapped pinned memory that a kernel on `stream` writes); checks the stream for errors,
+// and for a kernel that finished without signalling, every 4096 spins.
+template <class Done> int hv_poll(cudaStream_t stream, const char* who, Done done)
+{
+    for (unsigned long long spins = 1;; spins++) {
+        if (done()) break;
+        if ((spins & 0xfff) == 0) {
+            const cudaError_t q = cudaStreamQuery(stream);
+            if (q == cudaErrorNotReady) continue;
+            if (q != cudaSuccess) { hv_set_error("%s: %s while waiting for the result", who, cudaGetErrorString(q)); return HV_ERR_CUDA; }
+            if (done()) break;
+            hv_set_error("%s: the kernel finished without signalling its completion", who); return HV_ERR_STATE;
+        }
+    }
+    __atomic_thread_fence(__ATOMIC_ACQUIRE);
+    return HV_OK;
+}
 
 // kernels (pyramid.cu, lk.cu)
 cudaError_t hv_launch_pyr_fused(const HvPyrDesc* table, const unsigned short* idx, const uint8_t* const* src, const int* srcPitch,

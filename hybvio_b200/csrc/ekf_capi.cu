@@ -229,7 +229,7 @@ static int ekf_alloc(hv_ctx* c, const hv_ekf_params* prm, hv_ekf** out)
     e->cworkSide = p; p += cworkD; e->resSide = p; p += resD; e->d_opres = p; p += 4 * HV_RUN_MAX_OPS;
     e->d_mean20 = p;
     e->b.N = e->N; e->b.trail = e->trail; e->b.mapDim = e->mapDim;
-    err = cudaMallocHost(&e->h_pin, (e->inDoubles + N + 8 + EKF_RES_STRIDE * EKF_MAX_BATCH) * sizeof(double));
+    err = cudaMallocHost(&e->h_pin, (e->inDoubles + N + 8) * sizeof(double));
     if (err != cudaSuccess) { cudaFree(e->d_block); delete e; hv_set_error("hv_ekf_create: cudaMallocHost failed"); return HV_ERR_OOM; }
     if (cudaEventCreateWithFlags(&e->evStaged, cudaEventDisableTiming) != cudaSuccess) { cudaFree(e->d_block); cudaFreeHost(e->h_pin); delete e; hv_set_error("hv_ekf_create: cudaEventCreate failed"); return HV_ERR_CUDA; }
     err = cudaHostAlloc(&e->h_sig, 4 * sizeof(double) * (EKF_MAX_BATCH + 1), cudaHostAllocMapped);
@@ -680,24 +680,12 @@ static int staging_release(hv_ekf* e)      // call right after the H2D copy has 
 // Waits for `count` result slots of the mapped buffer to carry sequence number seq (written by ekf_report).
 static int poll_results(hv_ekf* e, int count, double seq, const char* who)
 {
-    cudaStream_t s = e->ctx->stream;
-    for (int i = 0; i < count; i++) {
-        volatile double* flag = e->h_sig + 4 * i + 3;
-        for (unsigned long long spins = 1;; spins++) {
-            if (*flag == seq) break;
-            if ((spins & 0xfff) == 0) {
-                const cudaError_t q = cudaStreamQuery(s);
-                if (q == cudaErrorNotReady) continue;
-                if (q != cudaSuccess) { hv_set_error("%s: %s while waiting for the result", who, cudaGetErrorString(q)); return HV_ERR_CUDA; }
-                if (*flag == seq) break;
-                hv_set_error("%s: the kernel finished without reporting its result", who); return HV_ERR_STATE;
-            }
-        }
-    }
-    __atomic_thread_fence(__ATOMIC_ACQUIRE);
-    return HV_OK;
+    int ready = 0;
+    return hv_poll(e->ctx->stream, who, [&] {
+        while (ready < count && ((volatile double*)e->h_sig)[4 * ready + 3] == seq) ready++;
+        return ready == count;
+    });
 }
-static bool ekf_polling() { static const bool on = getenv("HV_NO_POLL") == nullptr; return on; }
 
 static int visual_host(hv_ekf* e, const char* who, const double* H, int n, int l, const double* f, const double* y, double r,
                        double rmseThr, int mode, int* vuStatus, double* chi2, double* mOut)
@@ -732,12 +720,12 @@ static int visual_host(hv_ekf* e, const char* who, const double* H, int n, int l
     rc = staging_release(e);
     if (rc != HV_OK) return rc;
     a.H = e->d_in; a.f = e->d_in + nl; a.y = e->d_in + nl + n;
-    const bool polled = ekf_polling() && mode != EKF_MODE_UPDATE && !mOut;
+    const bool polled = mode != EKF_MODE_UPDATE && !mOut;
     if (polled) { a.sig = e->d_sig; a.sigSeq = (e->sigSeq += 1.0); }
     // A pure check speculates: the same kernel goes on to compute the update the reference issues for an INLIER (with the noise level of the
     // previous updateVisualTrack) into P2 / m2, while the host already has the decision; P and m stay as they are. Only the cluster kernel
     // has the second buffers (the single-CTA kernel would update P in place).
-    const bool speculate = polled && mode == EKF_MODE_CHECK && e->specEnabled && e->specR > 0.0 && !a.skipChi2 && a.rmseThr < 0.0 && r > 0.0 &&
+    const bool speculate = mode == EKF_MODE_CHECK && e->specEnabled && e->specR > 0.0 && !a.skipChi2 && a.rmseThr < 0.0 && r > 0.0 &&
                            ekf_cluster2_fits(n, l, e->N, false);
     if (speculate) {
         int rcj = join_side(e);
@@ -990,8 +978,7 @@ static int flush_checks(hv_ekf* e, const hv_ekf_op* ops, int first, int count, b
         if (rc != HV_OK) return rc;
     }
     a.b = e->b; a.noiseScale = e->noiseScale;
-    const bool polled = host && ekf_polling();           // every item fits the cluster kernel (batchable_check)
-    if (polled) { a.sig = e->d_sig; a.sigSeq = (e->sigSeq += 1.0); }
+    if (host) { a.sig = e->d_sig; a.sigSeq = (e->sigSeq += 1.0); }       // every item fits the cluster kernel (batchable_check)
     if (!host && first + count <= HV_RUN_MAX_OPS) a.slot = e->d_opres + 4 * first;      // hv_ekf_run_device_results
     if (augDiscarded >= 0) {
         int rcj = join_side(e);                            // (checks of the previous list read the buffers this augmentation writes)
@@ -1024,22 +1011,13 @@ static int flush_checks(hv_ekf* e, const hv_ekf_op* ops, int first, int count, b
         augment_done(e);
     } else HV_CUDA(ekf_launch_check_batch2(a, b, s));
     e->ctx->launches++;
-    if (polled) {
+    if (host) {
         int rc = poll_results(e, count, a.sigSeq, "hv_ekf_run");
         if (rc != HV_OK) return rc;
         for (int i = 0; i < count; i++) {
             if (vuStatus) vuStatus[first + i] = (int)e->h_sig[4 * i];
             if (chi2) chi2[first + i] = e->h_sig[4 * i + 1];
             if (e->h_sig[4 * i + 2] != 0.0) { hv_set_error("hv_ekf_run: op %d: innovation covariance not positive definite", first + i); return HV_ERR_STATE; }
-        }
-    } else if (host) {
-        double* hout = e->h_pin + e->inDoubles + e->N + 8;
-        HV_CUDA(cudaMemcpyAsync(hout, e->b.res, sizeof(double) * EKF_RES_STRIDE * count, cudaMemcpyDeviceToHost, s));
-        HV_CUDA(cudaStreamSynchronize(s));
-        for (int i = 0; i < count; i++) {
-            if (vuStatus) vuStatus[first + i] = (int)hout[EKF_RES_STRIDE * i];
-            if (chi2) chi2[first + i] = hout[EKF_RES_STRIDE * i + 1];
-            if (hout[EKF_RES_STRIDE * i + 2] != 0.0) { hv_set_error("hv_ekf_run: op %d: innovation covariance not positive definite", first + i); return HV_ERR_STATE; }
         }
     }
     return HV_OK;
@@ -1493,11 +1471,9 @@ int hv_ekf_run_host(hv_ekf* e, const hv_ekf_op* ops, int nops, int* vuStatus, do
 {
     EKF_ENTER(e, "hv_ekf_run_host");
     if (!ops || nops < 0) { hv_set_error("hv_ekf_run: invalid argument"); return HV_ERR_INVALID; }
-    if (ekf_polling()) {          // HV_NO_POLL=1: the per-op path (one round trip per measurement) instead, for A/B
-        int handled = 0;
-        const int rc = run_ops_host_async(e, ops, nops, vuStatus, chi2, mOut, &handled);
-        if (handled || rc != HV_OK) return rc;
-    }
+    int handled = 0;
+    const int rc = run_ops_host_async(e, ops, nops, vuStatus, chi2, mOut, &handled);
+    if (handled || rc != HV_OK) return rc;
     return run_ops(e, ops, nops, true, vuStatus, chi2, mOut);
 }
 
@@ -1984,26 +1960,15 @@ int hv_ekf_visual_track(hv_ekf* e, const hv_track_model* t, double r, double rms
     int rc = visual_args(e, who, t->rows, t->cols, r, rmseThr, mode, a);
     if (rc != HV_OK) return rc;
     a.H = t->d_H; a.f = t->d_f; a.y = t->d_y;
-    const bool polled = ekf_polling() && mode != EKF_MODE_UPDATE;
-    if (polled) { a.sig = e->d_sig; a.sigSeq = (e->sigSeq += 1.0); }
+    if (mode != EKF_MODE_UPDATE) { a.sig = e->d_sig; a.sigSeq = (e->sigSeq += 1.0); }
     rc = launch_update(e, a);
     if (rc != HV_OK) return rc;
     if (mode == EKF_MODE_UPDATE) return HV_OK;                   // asynchronous
-    cudaStream_t s = e->ctx->stream;
-    double st[3];
-    if (polled) {
-        rc = poll_results(e, 1, a.sigSeq, who);
-        if (rc != HV_OK) return rc;
-        st[0] = e->h_sig[0]; st[1] = e->h_sig[1]; st[2] = e->h_sig[2];
-    } else {
-        double* hout = e->h_pin + e->inDoubles;
-        HV_CUDA(cudaMemcpyAsync(hout, e->b.res, 3 * sizeof(double), cudaMemcpyDeviceToHost, s));
-        HV_CUDA(cudaStreamSynchronize(s));
-        st[0] = hout[0]; st[1] = hout[1]; st[2] = hout[2];
-    }
-    if (vuStatus) *vuStatus = (int)st[0];
-    if (chi2) *chi2 = st[1];
-    if (st[2] != 0.0) { hv_set_error("%s: innovation covariance not positive definite", who); return HV_ERR_STATE; }
+    rc = poll_results(e, 1, a.sigSeq, who);
+    if (rc != HV_OK) return rc;
+    if (vuStatus) *vuStatus = (int)e->h_sig[0];
+    if (chi2) *chi2 = e->h_sig[1];
+    if (e->h_sig[2] != 0.0) { hv_set_error("%s: innovation covariance not positive definite", who); return HV_ERR_STATE; }
     return HV_OK;
 }
 

@@ -92,10 +92,9 @@ __device__ __forceinline__ void hv_gftt_cell(const GfttArgs& a, int cellX, int c
         out[0] = found ? (float)(x0 + bidx % bs) : 0.0f;               // the reference leaves (0, 0) when no pixel of the cell qualifies
         out[1] = found ? (float)(y0 + bidx / bs) : 0.0f;
         out[2] = best;
-        if (a.hostFlag) {
+        if (a.done.hostFlag) {
             __threadfence_system();
-            const unsigned old = atomicAdd(a.doneCounter, 1u);
-            if (old + 1u == a.doneTarget) { __threadfence_system(); *a.hostFlag = a.seq; }
+            hv_signal_done(a.done);
         }
     }
 }

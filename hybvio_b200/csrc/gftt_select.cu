@@ -110,13 +110,10 @@ __device__ __forceinline__ void hv_gftt_select_list(const GfttSelectArgs& a)
         a.out[2 * i] = x; a.out[2 * i + 1] = y;
     }
     if (tid == 0) *a.count = count;
-    if (a.hostFlag) {
+    if (a.done.hostFlag) {
         __threadfence_system();
         __syncthreads();
-        if (tid == 0) {
-            const unsigned old = atomicAdd(a.doneCounter, 1u);
-            if (old + 1u == a.doneTarget) { __threadfence_system(); *a.hostFlag = a.seq; }
-        }
+        if (tid == 0) hv_signal_done(a.done);
     }
 }
 

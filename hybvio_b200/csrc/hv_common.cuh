@@ -35,6 +35,23 @@ __host__ __device__ __forceinline__ int hv_reflect101(int p, int len)
     return p;
 }
 
+// Completion signal of a host-buffer launch whose results land in mapped pinned host memory: every CTA makes its results visible
+// system-wide (__threadfence_system) and calls hv_signal_done; the last of the launch's `target` counts stores seq into *hostFlag,
+// which the host polls instead of a D2H copy + stream synchronisation. hostFlag NULL: no signal.
+struct HvDoneSignal {
+    unsigned* counter;
+    unsigned target, seq;
+    volatile unsigned* hostFlag;
+};
+
+#if defined(__CUDACC__) || defined(HV_EMU)      // (a plain host compiler that reads the argument blocks has no device intrinsics)
+__device__ __forceinline__ void hv_signal_done(const HvDoneSignal& d)
+{
+    const unsigned old = atomicAdd(d.counter, 1u);
+    if (old + 1u == d.target) { __threadfence_system(); *d.hostFlag = d.seq; }
+}
+#endif
+
 // ---- Lucas-Kanade launch description (lk.cu)
 #define LK_WARPS_PER_CTA 4
 #define LK_MAX_JOBS 8
@@ -58,12 +75,7 @@ struct LkLaunch {
     int maxIter;                // already clamped to [0,100]
     double eps2;                // already clamped and squared
     float minEig;
-    // Completion signal for the host-buffer API (single job, CTA-per-feature kernel): every CTA bumps *doneCounter after
-    // its results are visible system-wide; the one that reaches doneTarget stores seq into *hostFlag (mapped pinned host
-    // memory), which the host polls instead of a D2H copy + stream synchronisation. NULL: no signal.
-    unsigned* doneCounter;
-    unsigned doneTarget, seq;
-    volatile unsigned* hostFlag;
+    HvDoneSignal done;          // host-buffer API (single job, CTA-per-feature kernel): one count per CTA
     int prefetch;               // CTA-per-feature kernel: request the search region of a level with cp.async before the template patch is loaded
 };
 
@@ -80,7 +92,7 @@ struct GfttArgs {
     float k0, k1;             // [1 2 1] * scale as the fp32 kernel OpenCV builds (k0 = 2 s, k1 = s)
     float minResponse;
     float* kp;                // cellsX * cellsY * (x, y, response * 16); may be mapped pinned host memory
-    unsigned* doneCounter; unsigned doneTarget, seq; volatile unsigned* hostFlag;      // polled completion (like the LK kernel), optional
+    HvDoneSignal done;        // host-buffer API: one count per CTA
 };
 
 cudaError_t hv_launch_gftt(const GfttArgs& a, cudaStream_t stream);
@@ -101,7 +113,7 @@ __host__ __device__ __forceinline__ int hv_batch_job(const int* first, int b)
     return j;
 }
 struct GfttBatchArgs {
-    GfttArgs job[HV_CORNER_BATCH_MAX];        // hostFlag NULL
+    GfttArgs job[HV_CORNER_BATCH_MAX];        // done.hostFlag NULL
     int first[HV_CORNER_BATCH_MAX + 1];       // first CTA (cell) of job j in the flattened grid; first[njobs ..] = the grid
     int cellsX[HV_CORNER_BATCH_MAX];
 };
@@ -120,13 +132,13 @@ struct GfttSelectArgs {
     int pow2;                         // sort width: the smallest power of two >= nkp (>= 2)
     float* out; int capacity;         // (x, y) per slot; may be mapped pinned host memory
     int* count;                       // may be mapped pinned host memory
-    unsigned* doneCounter; unsigned doneTarget, seq; volatile unsigned* hostFlag;      // polled completion (like the LK kernel), optional
+    HvDoneSignal done;        // host-buffer API: one count per CTA
 };
 
 cudaError_t hv_launch_gftt_select(const GfttSelectArgs& a, cudaStream_t stream);
 
 struct GfttSelectBatchArgs {
-    GfttSelectArgs job[HV_CORNER_BATCH_MAX];  // CTA j is list j; hostFlag NULL
+    GfttSelectArgs job[HV_CORNER_BATCH_MAX];  // CTA j is list j; done.hostFlag NULL
 };
 static_assert(sizeof(GfttSelectBatchArgs) <= HV_KERNEL_PARAM_MAX, "select batch arguments exceed the kernel-parameter space");
 // maxPow2: the largest job[j].pow2, which sizes the dynamic shared memory of every CTA
@@ -141,14 +153,14 @@ struct SubpixArgs {
     int maxIters;                     // already clamped as cv::cornerSubPix does
     double eps2;                      // already clamped and squared
     float mask[(2 * HV_SUBPIX_MAX_HALF + 1) * (2 * HV_SUBPIX_MAX_HALF + 1)];    // (2 hh + 1) x (2 hw + 1), built on the host, zero zone applied
-    unsigned* doneCounter; unsigned doneTarget, seq; volatile unsigned* hostFlag;       // polled completion (like the LK kernel), optional
+    HvDoneSignal done;                // host-buffer API: one count per CTA
 };
 
 cudaError_t hv_launch_subpix(const SubpixArgs& a, cudaStream_t stream);
 
 struct SubpixJob { const uint8_t* gray; int pitch, w, h; float2* xy; int n; };
 struct SubpixBatchArgs {
-    SubpixArgs s;                             // window, criteria and mask of the whole batch (gray, xy, n and the flag unused)
+    SubpixArgs s;                             // window, criteria and mask of the whole batch (gray, xy, n and done unused)
     SubpixJob job[HV_CORNER_BATCH_MAX];
     int first[HV_CORNER_BATCH_MAX + 1];       // first CTA (point) of job j in the flattened grid; first[njobs ..] = the grid
 };

@@ -491,10 +491,9 @@ __global__ void __launch_bounds__(NW * 32) hv_lk_cta_kernel(LkLaunch L)
             if (outPt.x < 0.0f || outPt.x >= W || outPt.y < 0.0f || outPt.y >= H) ts = 4;
             job.trackStatus[f] = ts;
         }
-        if (L.hostFlag) {       // results may live in mapped host memory: make them visible, count, last one raises the flag
+        if (L.done.hostFlag) {  // results may live in mapped host memory: make them visible, count, last one raises the flag
             __threadfence_system();
-            const unsigned old = atomicAdd(L.doneCounter, 1u);
-            if (old + 1u == L.doneTarget) { __threadfence_system(); *L.hostFlag = L.seq; }
+            hv_signal_done(L.done);
         }
     }
 }

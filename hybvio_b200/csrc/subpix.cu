@@ -136,10 +136,9 @@ __global__ void __launch_bounds__(32) hv_subpix_kernel(const __grid_constant__ S
     const float2 r = hv_subpix_corner(a, a.gray, a.pitch, a.w, a.h, a.xy + blockIdx.x);
     if (threadIdx.x == 0) {
         a.xy[blockIdx.x] = r;
-        if (a.hostFlag) {
+        if (a.done.hostFlag) {
             __threadfence_system();
-            const unsigned old = atomicAdd(a.doneCounter, 1u);
-            if (old + 1u == a.doneTarget) { __threadfence_system(); *a.hostFlag = a.seq; }
+            hv_signal_done(a.done);
         }
     }
 }

@@ -34,7 +34,7 @@ int main(int argc, char** argv)
         a.pow2 = 2; while (a.pow2 < nkp) a.pow2 *= 2;
         a.out = out.data(); a.capacity = cap; a.count = &count;
         unsigned done = 0, flag = 0;
-        a.doneCounter = &done; a.doneTarget = 1; a.seq = 9; a.hostFlag = &flag;
+        a.done = HvDoneSignal{&done, 1, 9, &flag};
         std::vector<unsigned long long> smem((size_t)a.pow2 + 2, 0x5A5A5A5A5A5A5A5Aull);
         emu_dynamic_smem = (unsigned char*)smem.data();
         gridDim.x = gridDim.y = gridDim.z = 1;

@@ -75,7 +75,7 @@ static int run(const char* name, int w, int h, int kind, int hw, int hh, int zw,
     a.eps2 = e * e;
     orc_subpix_mask(hw, hh, zw, zh, a.mask);
     unsigned done = 0, flag = 0;
-    a.doneCounter = &done; a.doneTarget = (unsigned)n; a.seq = 7; a.hostFlag = &flag;
+    a.done = HvDoneSignal{&done, (unsigned)n, 7, &flag};
     std::vector<unsigned char> smem(hv_subpix_smem_bytes(hw, hh) + 64, 0x5A);
     emu_dynamic_smem = (unsigned char*)(((uintptr_t)smem.data() + 15) & ~(uintptr_t)15);
     gridDim.x = n; gridDim.y = gridDim.z = 1;

@@ -198,6 +198,82 @@ def test_host_list_of_checks_across_batch_splits(hv, oracle_lk, trail, ms):
     e.close()
 
 
+HV_RUN_MAX_OPS = 256
+
+
+def _host_frames(capi, N, frames, seed):
+    """`frames` frames of a host op list: 10 IMU predicts, one check + update, 8 outlier checks (every third a gross outlier), symmetrise,
+    augment. Returns the ops, the ops per frame and the arrays they point into."""
+    rng, irng = np.random.RandomState(seed), np.random.RandomState(seed + 1)
+    per = 10 + 1 + 8 + 2
+    ops = (capi.EkfOp * (per * frames))()
+    keep, t, k = [], 0.0, 0
+    for fr in range(frames):
+        for s_ in range(10):
+            t += 0.005
+            g, a = ekf_script.imu_sample(irng, 10 * fr + s_ + 1)
+            ops[k].kind, ops[k].t = capi.OP_PREDICT, t
+            for q in range(3):
+                ops[k].gyro[q], ops[k].acc[q] = g[q], a[q]
+            k += 1
+        for c in range(9):
+            H, f, y = ekf_script.visual_measurement(rng, (8, 20)[c % 2], N, 40.0 if c % 3 == 2 else 0.02)
+            H, f, y = np.asfortranarray(H), np.ascontiguousarray(f), np.ascontiguousarray(y)
+            keep += [H, f, y]
+            op = ops[k]
+            op.kind, op.n, op.l, op.mode, op.r, op.rmse_thr = capi.OP_VISUAL, H.shape[0], H.shape[1], 2 if c == 0 else 0, ekf_script.VISUAL_R, -1.0
+            op.H, op.f, op.y = H.ctypes.data, f.ctypes.data, y.ctypes.data
+            k += 1
+        ops[k].kind = capi.OP_SYMMETRIZE
+        ops[k + 1].kind, ops[k + 1].index = capi.OP_AUGMENT, -1
+        k += 2
+    return ops, per, keep
+
+
+def test_host_list_longer_than_one_async_list_matches_shorter_lists(hv):
+    """hv_ekf_run_host with more ops than HV_RUN_MAX_OPS cannot take the asynchronous path (one synchronisation per list) and runs op by op:
+    each check batch stages its inputs and polls its results, each check + update goes through the single-measurement host call. 15
+    frames (315 ops) in one call, and the same ops in calls of at most 256 ops split at frame boundaries (each taken by the asynchronous
+    path) on a clone of the same filter: statuses, chi2, the returned mean and the final m and P bit for bit."""
+    from hybvio_b200 import capi
+    lib = capi.load()
+    one = capi.Ekf(hv, _params(20, 0))
+    one.initialize_orientation(ekf_script.imu_sample(np.random.RandomState(1), 0)[1])
+    split = one.clone()
+    frames = 15
+    ops, per, keep = _host_frames(capi, one.N, frames, 9)
+    nops = per * frames
+    assert nops > HV_RUN_MAX_OPS
+    for i in range(nops):        # every check joins a check batch on both paths
+        assert ops[i].kind != capi.OP_VISUAL or ops[i].mode != 0 or K.kernel_path(ops[i].n, ops[i].l, one.N)[0] == "cluster"
+
+    def host_times(e):           # {issue, wait, total, ops} of the last list the asynchronous path ran
+        t = (ctypes.c_double * 4)()
+        assert lib.hv_ekf_debug_host_times(e.h, t) == 0
+        return list(t)
+
+    before = host_times(one)
+    st, c2, m = one.run_host(ops, nops, want_m=True)
+    assert host_times(one) == before, "the asynchronous path took a list longer than it accepts"
+
+    step = HV_RUN_MAX_OPS // per * per
+    parts = []
+    for start in range(0, nops, step):
+        cnt = min(step, nops - start)
+        chunk = (capi.EkfOp * cnt).from_address(ctypes.addressof(ops) + start * ctypes.sizeof(capi.EkfOp))
+        parts.append(split.run_host(chunk, cnt, want_m=True))
+        assert host_times(split)[3] == cnt, f"ops {start}..{start + cnt}: not run by the asynchronous path"
+    visual = [i for i in range(nops) if ops[i].kind == capi.OP_VISUAL]
+    assert 0 in st[visual] and (st[visual] != 0).any()
+    assert np.array_equal(st, np.concatenate([p[0] for p in parts]))
+    assert np.array_equal(c2.view(np.uint64), np.concatenate([p[1] for p in parts]).view(np.uint64))
+    assert np.array_equal(m.view(np.uint64), parts[-1][2].view(np.uint64))
+    (m1, P1), (m2, P2) = one.download(), split.download()
+    assert np.array_equal(m1.view(np.uint64), m.view(np.uint64))
+    assert np.array_equal(m1.view(np.uint64), m2.view(np.uint64)) and np.array_equal(P1.view(np.uint64), P2.view(np.uint64))
+    one.close(); split.close()
+
+
 def _boundary_shapes():
     """One shape on each side of each cluster / single-CTA boundary (and of the shared / global tableau one)."""
     out = []

@@ -9,9 +9,8 @@ every chunk: the last frame's pyramids and LK outputs bit for bit, its check dec
 within the replay's rounding envelope. hv_e2e_run keeps its LK outputs and check results inside the driver: for it, the
 pyramids, the state and the returned pose are compared.
 
-The same 200 frames must leave the same bits whatever the schedule: one uninterrupted call, the chunks, HV_EKF_NO_PDL=1,
-HV_BENCH_NO_OVERLAP=1 (step_device) and HV_NO_POLL=1 (host-buffer drivers). Those switches are read once per process, so every
-configuration runs in a child process, once.
+The same 200 frames must leave the same bits whatever the schedule: one uninterrupted call, the chunks, HV_EKF_NO_PDL=1 and
+HV_BENCH_NO_OVERLAP=1 (step_device). Those switches are read once per process, so every configuration runs in a child process, once.
 
 Host-buffer and device families run the same kernels for the benchmark's list (see ekf_capi.cu: run_ops_host_async and run_ops
 both issue the IMU burst as one predict launch, every check + update through launch_update, and the 15 outlier checks as one
@@ -52,7 +51,6 @@ JOBS = {
     "default": ({}, [(d, "chunked") for d in DRIVERS + ("step_device_copy",)] + [(d, "one_call") for d in DRIVERS]),
     "no_pdl": ({"HV_EKF_NO_PDL": "1"}, [(d, "chunked") for d in DRIVERS]),
     "no_overlap": ({"HV_BENCH_NO_OVERLAP": "1"}, [("step_device", "chunked")]),
-    "no_poll": ({"HV_NO_POLL": "1"}, [(d, "chunked") for d in HOST_DRIVERS]),
 }
 LAUNCHES_PER_FRAME = {"default": 12, "no_pdl": 11}       # hv_dev_run: latency mode, throughput mode (HV_EKF_NO_PDL=1)
 

@@ -4,8 +4,6 @@ the padding slots set to HV_CORNER_NONE -- on the golden frames, over the detect
 max_tracks and previous corners, on crafted key points (stability, signed zeros, empty cells, the rounded distance, 1 .. 16384 key
 points), in the device chain detect -> select -> cornerSubPix -> stereo LK with one synchronisation, and the documented error codes."""
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -253,41 +251,3 @@ def test_error_codes(hv):
     assert hv.launches == before
     q.release(); other.close(); p.release(); big.release()
 
-
-_NO_POLL_CHILD = r"""
-import sys
-sys.path.insert(0, {root!r}); sys.path.insert(0, {tests!r})
-import numpy as np
-import gftt_select_common as gc
-from hybvio_b200 import capi, synth
-hv = capi.Context(0)
-out = []
-for k, cell in ((3, 32), (4, 8)):
-    img, _ = synth.stereo_frame(k, 752, 480)
-    p = hv.pyramid(752, 480, 31, 1)
-    p.build(np.ascontiguousarray(img))
-    for r, m in ((0, 150), (8, 150), (50, 7)):
-        out.append(p.gftt_corners(gc.prev_points(40, k, 752, 480), r, m, 3, cell))
-    p.release()
-np.savez({path!r}, *out)
-hv.close()
-"""
-
-
-@pytest.mark.gpu
-def test_no_poll_path_gives_the_same_lists(orc, tmp_path):
-    """HV_NO_POLL=1 (copy + stream synchronisation instead of the mapped block and its flag) in a child process: same lists."""
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    path = str(tmp_path / "nopoll.npz")
-    env = dict(os.environ, HV_NO_POLL="1")
-    r = subprocess.run([sys.executable, "-c", _NO_POLL_CHILD.format(root=root, tests=os.path.join(root, "tests"), path=path)], env=env,
-                       capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stdout + r.stderr
-    got = np.load(path)
-    i = 0
-    for k, cell in ((3, 32), (4, 8)):
-        img, _ = synth.stereo_frame(k, 752, 480)
-        kp = orc.collect(orc.response(img), cell, 1e-3)
-        for rad, m in ((0, 150), (8, 150), (50, 7)):
-            assert_list(got[f"arr_{i}"], orc.corners(kp, gc.prev_points(40, k, 752, 480), rad, m), f"HV_NO_POLL=1 cell {cell} r {rad}")
-            i += 1

@@ -2,10 +2,6 @@
 cv::cornerSubPix oracle (oracle/hv_oracle_subpix.c, itself bit-exact to cv2 with IPP off, test_oracle_subpix.py): every refined
 corner BIT-identical, over the same sweep of windows, zero zones, criteria, images and start points; on pyramids from hv_pyr_build,
 hv_pyr_build_batch with device sources and hv_ingest_frame with a remap; n = 0 .. 2000; the documented error codes."""
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 
@@ -178,32 +174,3 @@ def test_device_call_leaves_corners_outside_the_image_unchanged(hv, orc):
     assert np.array_equal(got[20:26].view(np.uint32), outside.view(np.uint32))
     p.release()
 
-
-_NO_POLL_CHILD = r"""
-import sys
-sys.path.insert(0, {root!r}); sys.path.insert(0, {tests!r})
-import numpy as np
-import subpix_common as sc
-from hybvio_b200 import capi
-hv = capi.Context(0)
-img = sc.images()["frame751"]
-p = hv.pyramid(img.shape[1], img.shape[0], 31, 1)
-p.build(np.ascontiguousarray(img))
-out = [p.subpix_refine(sc.points(img, win, seed=5), win, (1, 1), (3, 30, 0.01)) for win in [(2, 3), (5, 5), (15, 15)]]
-np.save({path!r}, np.concatenate(out))
-p.release(); hv.close()
-"""
-
-
-@pytest.mark.gpu
-def test_no_poll_path_gives_the_same_bits(hv, orc, tmp_path):
-    """HV_NO_POLL=1 (copy + stream synchronisation instead of the mapped block and its flag) in a child process: same bits."""
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    path = str(tmp_path / "nopoll.npy")
-    env = dict(os.environ, HV_NO_POLL="1")
-    r = subprocess.run([sys.executable, "-c", _NO_POLL_CHILD.format(root=root, tests=os.path.join(root, "tests"), path=path)], env=env,
-                       capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stdout + r.stderr
-    img = sc.images()["frame751"]
-    want = np.concatenate([orc.refine(img, sc.points(img, win, seed=5), win, (1, 1), (3, 30, 0.01)) for win in [(2, 3), (5, 5), (15, 15)]])
-    assert_bits(np.load(path), want, "HV_NO_POLL=1")
