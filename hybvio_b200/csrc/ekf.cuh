@@ -179,6 +179,10 @@ int ekf_cluster2_chunk_rows(int n, int l, int N);
 cudaError_t ekf_launch_update_cluster2(const EkfUpdateArgs& a, cudaStream_t s);
 // aug != NULL: one more cluster of the same launch runs the augmentation *aug (results into aug->specP / aug->specM)
 cudaError_t ekf_launch_check_batch2(const EkfUpdateArgs& a, const EkfCheckBatch& b, cudaStream_t s, const EkfUpdateArgs* aug = nullptr);
+// The state mean of the augmentation a (EKF_OP_AUGMENT) into a.specM on one CTA, bitwise what the cluster kernel writes there; its
+// covariance is left to a cluster launched elsewhere (flush_checks). Fits iff ekf_aug_mean_fits(a.b.N).
+bool ekf_aug_mean_fits(int N);
+cudaError_t ekf_launch_aug_mean(const EkfUpdateArgs& a, cudaStream_t s);
 // Group launches (hv_ekf_group_run_device): instance i of the launch runs dArgs[i], a fully resolved argument block in device memory;
 // hArgs is the host copy of the same blocks (launch shape: shared memory of the largest instance)
 cudaError_t ekf_launch_group_cluster2(const EkfUpdateArgs* hArgs, const EkfUpdateArgs* dArgs, int count, cudaStream_t s);

@@ -38,9 +38,11 @@ struct hv_ekf {
     cudaStream_t copyStream = nullptr;            // hv_ekf_run_host: the measurement inputs travel on their own stream, ahead of the kernels
     std::vector<cudaEvent_t> copyEvents;          // one per measurement group of a list (created on demand)
     double sigSeq = 0.0;
-    // hv_ekf_run_device: a run of outlier checks that is followed by the pose augmentation goes to a SIDE stream (the checks only read
-    // the state, the augmentation writes the second buffers, so nothing that follows on the main stream has to wait for them);
-    // they are joined before the next writer of the second buffers and before anything that hands results to the host
+    // hv_ekf_run_device in latency mode: a run of outlier checks that is followed by the pose augmentation goes to a SIDE stream together
+    // with the augmentation's covariance (one launch: the checks read (m, P), the augmentation cluster writes P2); the augmentation's mean
+    // is formed on the context's stream by one CTA (ekf_launch_aug_mean, into m2), so that the next frame's mean propagation and optical
+    // flow do not wait for the covariance. While sideBusy, P is on the side stream: join_side() makes the context's stream wait for it,
+    // and every consumer of P (or writer of the second buffers) calls it before it issues; readers of the mean alone do not.
     cudaEvent_t evFork = nullptr, evJoin = nullptr;       // (the stream itself belongs to the context: hv_ctx::sideStream)
     // After hv_ekf_predicted_mean_device the full launch of the IMU burst (covariance) goes to a stream of its own (hv_ctx::covStream):
     // whatever the caller issues next on the context's stream without touching the filter (the optical flow, when tracker and filter
@@ -50,6 +52,7 @@ struct hv_ekf {
     bool sideBusy = false;
     double* cworkSide = nullptr;            // exchange areas and result words of the clusters on the side stream
     double* resSide = nullptr;
+    double* mSide = nullptr;                // where the augmentation cluster on the side stream leaves its mean (N; read by nobody)
     double* d_opres = nullptr;              // hv_ekf_run_device: result words per op of the list (4 doubles each, HV_RUN_MAX_OPS)
     double* d_mean20 = nullptr;             // hv_ekf_predicted_mean: device scratch
     std::vector<unsigned char> lastVisual;  // per op of the last hv_ekf_run_device list: 1 = VISUAL (has result words)
@@ -154,6 +157,8 @@ static void update_settle(hv_ekf* e, EkfUpdateArgs& a)
 }
 static int launch_update(hv_ekf* e, EkfUpdateArgs& a)
 {
+    int rcj = join_side(e);
+    if (rcj != HV_OK) return rcj;
     update_settle(e, a);
     HV_CUDA(ekf_launch_update(a, e->ctx->stream));
     e->ctx->launches++;
@@ -169,7 +174,8 @@ static void fill_small(EkfUpdateArgs& a, int op, int n, int l, double Rdiag, int
 static int launch_ew(hv_ekf* e, int op, int ival0 = 0, const double* dv = nullptr, int ndv = 0)
 {
     EkfEwArgs a; memset(&a, 0, sizeof(a));
-    if (op == EKF_EW_UNAUGMENT || op == EKF_EW_TRANSFORM) { int rcj = join_side(e); if (rcj != HV_OK) return rcj; }   // out of place into P2
+    int rcj = join_side(e);                           // (UNAUGMENT / TRANSFORM: out of place into P2)
+    if (rcj != HV_OK) return rcj;
     e->epoch++;
     a.b = e->b; a.op = op; a.ival0 = ival0;
     for (int i = 0; i < ndv; i++) a.dval[i] = dv[i];
@@ -179,7 +185,9 @@ static int launch_ew(hv_ekf* e, int op, int ival0 = 0, const double* dv = nullpt
 }
 
 static void swap_P(hv_ekf* e) { double* t = e->b.P; e->b.P = e->b.P2; e->b.P2 = t; }
-// Outlier checks still running on the side stream read what are now the SECOND buffers: every writer of P2 / m2 waits for them first
+// The launch on the side stream writes P (the augmentation's covariance) and reads what are now the SECOND buffers: every consumer of P and
+// every writer of P2 / m2 on the context's stream waits for it first (the covariance launch of an IMU burst on its own stream waits for
+// evJoin itself, predict_launch)
 static int join_side(hv_ekf* e)
 {
     if (!e->sideBusy) return HV_OK;
@@ -217,7 +225,7 @@ static int ekf_alloc(hv_ctx* c, const hv_ekf_params* prm, hv_ekf** out)
     const size_t cworkD = (size_t)(EKF_MAX_BATCH + 1) * 10 * NN;       // one exchange area per cluster of a check batch (+ its augmentation)
     e->inDoubles = (size_t)EKF_MAX_BATCH * (NN + 2 * N);
     const size_t resD = (size_t)EKF_RES_STRIDE * (EKF_MAX_BATCH + 1);
-    const size_t total = N + NN + NN + workD + 2 * cworkD + EKF_SMALL_MAXN * EKF_SMALL_MAXL + 144 + 400 + 2 * resD + e->inDoubles + N + 4 * HV_RUN_MAX_OPS + 32;
+    const size_t total = N + NN + NN + workD + 2 * cworkD + EKF_SMALL_MAXN * EKF_SMALL_MAXL + 144 + 400 + 2 * resD + e->inDoubles + N + 4 * HV_RUN_MAX_OPS + 32 + N;
     cudaError_t err = cudaMalloc(&e->d_block, total * sizeof(double));
     if (err != cudaSuccess) { delete e; hv_set_error("hv_ekf_create: cudaMalloc failed: %s", cudaGetErrorString(err)); return HV_ERR_OOM; }
     cudaMemsetAsync(e->d_block, 0, total * sizeof(double), c->stream);
@@ -227,7 +235,8 @@ static int ekf_alloc(hv_ctx* c, const hv_ekf_params* prm, hv_ekf** out)
     e->d_in = p; p += e->inDoubles;
     e->m2 = p; p += N;
     e->cworkSide = p; p += cworkD; e->resSide = p; p += resD; e->d_opres = p; p += 4 * HV_RUN_MAX_OPS;
-    e->d_mean20 = p;
+    e->d_mean20 = p; p += 32;
+    e->mSide = p;
     e->b.N = e->N; e->b.trail = e->trail; e->b.mapDim = e->mapDim;
     err = cudaMallocHost(&e->h_pin, (e->inDoubles + N + 8) * sizeof(double));
     if (err != cudaSuccess) { cudaFree(e->d_block); delete e; hv_set_error("hv_ekf_create: cudaMallocHost failed"); return HV_ERR_OOM; }
@@ -312,6 +321,7 @@ int hv_ekf_clone(const hv_ekf* src, hv_ekf** out)
     HV_CUDA(cudaSetDevice(src->ctx->device));
     hv_ekf* e = nullptr;
     int rc = flush_pending(const_cast<hv_ekf*>(src));     // deferred work belongs to the state being copied
+    if (rc == HV_OK) rc = join_side(const_cast<hv_ekf*>(src));
     if (rc != HV_OK) return rc;
     rc = ekf_alloc(src->ctx, &src->prm, &e);
     if (rc != HV_OK) return rc;
@@ -352,6 +362,7 @@ int hv_ekf_set_first_sample_time(hv_ekf* e, double t)
 int hv_ekf_upload(hv_ekf* e, const double* m, const double* P)
 {
     EKF_ENTER(e, "hv_ekf_upload");
+    { int rcj = join_side(e); if (rcj != HV_OK) return rcj; }
     e->epoch++;
     const size_t N = e->N;
     if (m) HV_CUDA(cudaMemcpyAsync(e->b.m, m, sizeof(double) * N, cudaMemcpyHostToDevice, e->ctx->stream));
@@ -363,6 +374,7 @@ int hv_ekf_upload(hv_ekf* e, const double* m, const double* P)
 int hv_ekf_download(hv_ekf* e, double* m, double* P)
 {
     EKF_ENTER(e, "hv_ekf_download");
+    { int rcj = join_side(e); if (rcj != HV_OK) return rcj; }
     const size_t N = e->N;
     if (m) HV_CUDA(cudaMemcpyAsync(m, e->b.m, sizeof(double) * N, cudaMemcpyDeviceToHost, e->ctx->stream));
     if (P) HV_CUDA(cudaMemcpyAsync(P, e->b.P, sizeof(double) * N * N, cudaMemcpyDeviceToHost, e->ctx->stream));
@@ -373,6 +385,7 @@ int hv_ekf_download(hv_ekf* e, double* m, double* P)
 int hv_ekf_download_inertial(hv_ekf* e, double* m20, double* P20)
 {
     EKF_ENTER(e, "hv_ekf_download_inertial");
+    { int rcj = join_side(e); if (rcj != HV_OK) return rcj; }
     if (m20) HV_CUDA(cudaMemcpyAsync(m20, e->b.m, sizeof(double) * 20, cudaMemcpyDeviceToHost, e->ctx->stream));
     if (P20) HV_CUDA(cudaMemcpy2DAsync(P20, 20 * sizeof(double), e->b.P, e->N * sizeof(double), 20 * sizeof(double), 20,
                                        cudaMemcpyDeviceToHost, e->ctx->stream));
@@ -383,6 +396,7 @@ int hv_ekf_download_inertial(hv_ekf* e, double* m20, double* P20)
 int hv_ekf_set_inertial_state(hv_ekf* e, const double* m20, const double* P20)
 {
     EKF_ENTER(e, "hv_ekf_set_inertial_state");
+    { int rcj = join_side(e); if (rcj != HV_OK) return rcj; }
     if (!m20 || !P20) { hv_set_error("hv_ekf_set_inertial_state: NULL"); return HV_ERR_INVALID; }
     e->epoch++;
     HV_CUDA(cudaMemcpyAsync(e->b.m, m20, sizeof(double) * 20, cudaMemcpyHostToDevice, e->ctx->stream));
@@ -488,11 +502,13 @@ static int predict_launch(hv_ekf* e, EkfPredictArgs& a)
         }
         HV_CUDA(cudaEventRecord(e->evCovFork, c->stream));        // behind everything issued so far (earlier filter work, the mean launch)
         HV_CUDA(cudaStreamWaitEvent(c->covStream, e->evCovFork, 0));
+        if (e->sideBusy) HV_CUDA(cudaStreamWaitEvent(c->covStream, e->evJoin, 0));     // ... and behind the covariance on the side stream
         HV_CUDA(ekf_launch_predict(a, c->covStream));
         HV_CUDA(cudaEventRecord(e->evCov, c->covStream));
         e->covBusy = true;
     } else {
         int rc = join_cov(e);
+        if (rc == HV_OK) rc = join_side(e);
         if (rc != HV_OK) return rc;
         HV_CUDA(ekf_launch_predict(a, e->ctx->stream));
     }
@@ -838,8 +854,7 @@ int hv_ekf_augment(hv_ekf* e, int discarded)
     if (discarded < 0 || discarded >= e->trail) { hv_set_error("hv_ekf_augment: pose index %d out of range", discarded); return HV_ERR_INVALID; }
     EkfUpdateArgs a; augment_args(e, discarded, e->pendSym, a);  // a deferred symmetrisation rides along
     e->pendSym = false;
-    if (!ekf_cluster2_fits(a.n, a.l, e->N, true)) { int rcj = join_side(e); if (rcj != HV_OK) return rcj; }      // the single-CTA kernel shifts into P2
-    int rc = launch_update(e, a);   // shift into P2, update there, Joseph product back into P: no swap
+    int rc = launch_update(e, a);   // (single-CTA kernel: shift into P2, update there, Joseph product back into P: no swap)
     if (rc != HV_OK) return rc;
     augment_done(e);
     return HV_OK;
@@ -959,6 +974,7 @@ static int flush_checks(hv_ekf* e, const hv_ekf_op* ops, int first, int count, b
     cudaStream_t s = e->ctx->stream;
     EkfUpdateArgs a; EkfCheckBatch b;
     int rci = check_items(e, ops, first, count, a, b);
+    if (rci == HV_OK) rci = join_side(e);             // (the checks read P; an augmentation writes the buffers earlier checks read)
     if (rci != HV_OK) return rci;
     if (host) {
         int rc = staging_acquire(e);
@@ -981,17 +997,16 @@ static int flush_checks(hv_ekf* e, const hv_ekf_op* ops, int first, int count, b
     if (host) { a.sig = e->d_sig; a.sigSeq = (e->sigSeq += 1.0); }       // every item fits the cluster kernel (batchable_check)
     if (!host && first + count <= HV_RUN_MAX_OPS) a.slot = e->d_opres + 4 * first;      // hv_ekf_run_device_results
     if (augDiscarded >= 0) {
-        int rcj = join_side(e);                            // (checks of the previous list read the buffers this augmentation writes)
-        if (rcj != HV_OK) return rcj;
         EkfUpdateArgs aug; fused_augment_args(e, augDiscarded, augSym, aug);
         // HV_EKF_NO_PDL=1 (throughput mode, many sessions per GPU): nothing is launched early or beside the main stream
         static const bool latencyMode = getenv("HV_EKF_NO_PDL") == nullptr;
-        if (host || !latencyMode) {
+        if (host || !latencyMode || !ekf_aug_mean_fits(e->N)) {
             // results are wanted now (or: one stream per session): the augmentation is one more cluster of the checks' launch
             HV_CUDA(ekf_launch_check_batch2(a, b, s, &aug));
         } else {
-            // nothing goes back to the host: the checks leave the main stream altogether (fork -> side stream), the augmentation and
-            // whatever follows it (the next frame's IMU burst, its visual updates) run beside them
+            // nothing goes back to the host: the checks and the augmentation's covariance leave the main stream (fork -> side stream, one
+            // launch, P2 written there), and the augmentation's mean is formed on the main stream by one CTA (m2): the next frame's mean
+            // propagation and optical flow, which read the mean only, run beside the covariance; its consumers of P join the side stream
             if (!e->ctx->sideStream) HV_CUDA(cudaStreamCreateWithFlags(&e->ctx->sideStream, cudaStreamNonBlocking));
             if (!e->evFork) {
                 HV_CUDA(cudaEventCreateWithFlags(&e->evFork, cudaEventDisableTiming));
@@ -1001,11 +1016,13 @@ static int flush_checks(hv_ekf* e, const hv_ekf_op* ops, int first, int count, b
             HV_CUDA(cudaEventRecord(e->evFork, s));
             HV_CUDA(cudaStreamWaitEvent(side, e->evFork, 0));
             a.b.cwork = e->cworkSide; a.b.res = e->resSide;
-            HV_CUDA(ekf_launch_check_batch2(a, b, side));
+            EkfUpdateArgs augCov = aug;                   // the cluster's mean goes to a scratch buffer: m2 has one writer, the kernel below
+            augCov.b.cwork = e->cworkSide; augCov.b.res = e->resSide; augCov.specM = e->mSide;
+            HV_CUDA(ekf_launch_check_batch2(a, b, side, &augCov));
             HV_CUDA(cudaEventRecord(e->evJoin, side));
             e->sideBusy = true;
             e->ctx->launches++;
-            HV_CUDA(ekf_launch_update(aug, s));
+            HV_CUDA(ekf_launch_aug_mean(aug, s));
         }
         adopt_second_buffers(e);
         augment_done(e);
@@ -1155,10 +1172,10 @@ static int run_ops_host_async(hv_ekf* e, const hv_ekf_op* ops, int nops, int* vu
             int disc = -1; bool sym = false;
             const int extra = batch ? augment_follows(e, ops, nops, i + cnt, &disc, &sym) : 0;
             if (cnt > 1 || extra) {
+                rc = join_side(e);
+                if (rc != HV_OK) return rc;
                 a.b = e->b; a.noiseScale = e->noiseScale;
                 if (extra) {
-                    rc = join_side(e);
-                    if (rc != HV_OK) return rc;
                     EkfUpdateArgs aug; augment_args(e, disc, sym, aug);
                     aug.noiseScale = e->noiseScale; aug.specP = e->b.P2; aug.specM = e->m2;
                     HV_CUDA(ekf_launch_check_batch2(a, b, s, &aug));
@@ -1791,6 +1808,7 @@ int hv_ekf_visual_tracks(hv_ekf* e, const hv_track_obs* tracks, int ntracks, con
                          int* successfulUpdates)
 {
     EKF_ENTER(e, "hv_ekf_visual_tracks");
+    { int rcj = join_side(e); if (rcj != HV_OK) return rcj; }
     const char* who = "hv_ekf_visual_tracks";
     if (!p || !out) { hv_set_error("%s: invalid argument", who); return HV_ERR_INVALID; }
     VisualChain ch;
@@ -1870,6 +1888,7 @@ int hv_ekf_group_visual_tracks(hv_ekf* const* ekfs, int count, const hv_track_ob
     for (int f = 0; f < count; f++) {
         if (ntracks[f] == 0) continue;
         int rc = flush_pending(ekfs[f]);                 // (EKF_ENTER: work queued by earlier calls goes first)
+        if (rc == HV_OK) rc = join_side(ekfs[f]);
         if (rc == HV_OK) rc = chain_begin(ekfs[f], whoF[f].c_str(), tracks[f], ntracks[f], &params[f], ch[f]);
         if (rc != HV_OK) return rc;
         winEnd[f] = chain_window(ch[f]);

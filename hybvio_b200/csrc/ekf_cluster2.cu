@@ -63,6 +63,13 @@ __global__ void __launch_bounds__(EK2_NT) ekf_check_batch_cluster2_kernel(EkfUpd
 }
 static_assert(2 * sizeof(EkfUpdateArgs) + sizeof(EkfCheckBatch) <= 4096, "ekf_check_batch_cluster2_kernel: arguments beyond 4 KB of parameter space");
 
+// The state mean of the pose augmentation on one CTA (ek2_aug_mean_cta), while a cluster elsewhere forms the covariance
+__global__ void __launch_bounds__(EK2_NT) ekf_aug_mean_kernel(EkfUpdateArgs a)
+{
+    extern __shared__ __align__(16) double ek2_sm[];
+    ek2_aug_mean_cta(a, ek2_sm);
+}
+
 // Group launch (hv_ekf_group_run_device): cluster i runs args[i], an instance of any filter of the group. The blocks live in device
 // memory (hundreds of clusters do not fit the parameter space); no cluster waits for another, so a grid of many clusters runs in waves.
 __global__ void __launch_bounds__(EK2_NT) ekf_group_cluster2_kernel(const EkfUpdateArgs* __restrict__ args)
@@ -149,6 +156,27 @@ cudaError_t ekf_launch_check_batch2(const EkfUpdateArgs& a, const EkfCheckBatch&
     clusters += (b.compact + EK2_C - 1) / EK2_C;
     if (aug) { const size_t v = ek2_smem_bytes(aug->n, aug->l, a.b.N, true); if (v > smem) smem = v; }
     return ek2_launch(ekf_check_batch_cluster2_kernel, clusters, smem, s, a, b, aug ? *aug : a);
+}
+
+bool ekf_aug_mean_fits(int N)
+{
+    return N <= EK2_MAXN && ek2_aug_mean_smem_bytes(EKF_POSE, EKF_CAM + EKF_POSE, N) <= EK2_SMEM_LIMIT;
+}
+
+cudaError_t ekf_launch_aug_mean(const EkfUpdateArgs& a, cudaStream_t s)
+{
+    static bool seen[64];
+    if (hv_first_use_on_device(seen)) {
+        cudaError_t e = cudaFuncSetAttribute(ekf_aug_mean_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)EK2_SMEM_LIMIT);
+        if (e != cudaSuccess) return e;
+    }
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(1); cfg.blockDim = dim3(EK2_NT); cfg.dynamicSmemBytes = ek2_aug_mean_smem_bytes(a.n, a.l, a.b.N); cfg.stream = s;
+    cudaLaunchAttribute at[1];
+    static const bool pdl = getenv("HV_EKF_NO_PDL") == nullptr;          // (as ek2_launch)
+    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = at; cfg.numAttrs = pdl ? 1 : 0;
+    return cudaLaunchKernelEx(&cfg, ekf_aug_mean_kernel, a);
 }
 
 cudaError_t ekf_launch_group_cluster2(const EkfUpdateArgs* hArgs, const EkfUpdateArgs* dArgs, int count, cudaStream_t s)

@@ -113,9 +113,9 @@ int hv_dev_run(hv_ctx* trk, hv_ctx* ekf_ctx, hv_pyr** pyr, hv_ekf* ekf, const fl
                uint8_t* d_status, int32_t* d_ts, int n, const hv_dev_frame* frames, int nframes, float* elapsed_ms)
 {
     // Stream sa (the tracker context's): pyramid builds only. Stream sb (the filter context's): the WHOLE dependent chain of a frame --
-    // mean propagation -> optical flow (hv_lk_track_device_on_stream) -> visual updates -> augmentation -- so that no step of it waits
-    // for a cross-stream event that has not fired long ago. Beside it, on streams of the library: the covariance part of the IMU burst
-    // and the outlier checks that precede the augmentation.
+    // mean propagation -> optical flow (hv_lk_track_device_on_stream) -> visual updates -> the augmentation's mean -- so that no step of it
+    // waits for a cross-stream event that has not fired long ago. Beside it, on streams of the library: the covariance part of the IMU
+    // burst, and the outlier checks that precede the augmentation together with the augmentation's covariance.
     hv_pyr* p[4] = {pyr[0], pyr[1], pyr[2], pyr[3]};
     cudaStream_t sa = (cudaStream_t)hv_ctx_stream(trk), sb = (cudaStream_t)hv_ctx_stream(ekf_ctx);
     cudaEvent_t e0, e1, evPyr, evLk;
