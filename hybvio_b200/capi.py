@@ -102,6 +102,19 @@ class GoodFeaturesJob(ctypes.Structure):
 CORNER_BATCH_MAX = 64   # HV_CORNER_BATCH_MAX
 
 
+class EssentialJob(ctypes.Structure):
+    """hv_essential_job: one session's correspondences, intrinsics and outputs in the batched essential-matrix RANSAC (see
+    essential_job)"""
+    _fields_ = [("d_xy1", c_void_p), ("d_xy2", c_void_p), ("d_status", c_void_p), ("n", c_int),
+                ("fx", c_double), ("fy", c_double), ("cx", c_double), ("cy", c_double),
+                ("d_E", c_void_p), ("d_nsol", c_void_p), ("d_mask", c_void_p), ("d_inliers", c_void_p)]
+
+
+ESSENTIAL_BATCH_MAX = 64       # HV_ESSENTIAL_BATCH_MAX
+ESSENTIAL_MAX_POINTS = 4096    # HV_ESSENTIAL_MAX_POINTS
+ESSENTIAL_MAX_ITERS = 4096     # HV_ESSENTIAL_MAX_ITERS
+
+
 class IngestJob(ctypes.Structure):
     """hv_ingest_job: one frame of hv_ingest_frames (see ingest_job)"""
     _fields_ = [("ing", c_void_p), ("src", c_void_p), ("stride_bytes", c_size_t), ("channels", c_int), ("coeff", c_void_p),
@@ -164,6 +177,10 @@ def load():
     lib.hv_good_features.argtypes = [c_void_p, c_void_p, c_int, c_int, c_double, c_double, c_void_p, c_size_t, c_void_p, c_void_p, c_int, c_void_p]
     lib.hv_good_features_device.argtypes = lib.hv_good_features.argtypes
     lib.hv_good_features_batch_device.argtypes = [c_void_p, ctypes.POINTER(GoodFeaturesJob), c_int, c_int, c_double, c_double]
+    lib.hv_find_essential.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_double, c_double, c_double, c_double, c_double,
+                                      c_double, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
+    lib.hv_find_essential_device.argtypes = lib.hv_find_essential.argtypes
+    lib.hv_find_essential_batch_device.argtypes = [c_void_p, ctypes.POINTER(EssentialJob), c_int, c_double, c_double, c_int]
     _bind_ekf(lib)
     _lib = lib
     return lib
@@ -392,6 +409,37 @@ class Context:
         check(self.lib.hv_good_features_batch_device(self.h, J, len(jobs), block_size, quality_level, min_distance),
               "hv_good_features_batch_device")
 
+    # ---- cv::findEssentialMat(..., RANSAC, prob, threshold, max_iters): one launch per call
+    def find_essential(self, xy1, xy2, fx, fy, cx, cy, prob=0.999, threshold=1.0, max_iters=1000, status=None):
+        """hv_find_essential on host arrays: xy1, xy2 (n, 2) float32 (converted), status (n,) uint8 or None. Returns (E, mask) as
+        cv2.findEssentialMat returns them: E (nsol, 3, 3) float64 row-major (nsol 0 where cv2 returns None), mask (n,) uint8."""
+        a = np.ascontiguousarray(xy1, np.float32).reshape(-1, 2)
+        b = np.ascontiguousarray(xy2, np.float32).reshape(-1, 2)
+        if a.shape != b.shape:
+            raise ValueError(f"xy1 {a.shape} and xy2 {b.shape} differ")
+        n = a.shape[0]
+        st = None if status is None else np.ascontiguousarray(status, np.uint8)
+        if st is not None and st.shape != (n,):
+            raise ValueError(f"status {st.shape} is not ({n},)")
+        E = np.zeros(90, np.float64)
+        mask = np.zeros(max(n, 1), np.uint8)
+        nsol, inl = ctypes.c_int(), ctypes.c_int()
+        check(self.lib.hv_find_essential(self.h, _ptr(a), _ptr(b), _ptr(st), n, fx, fy, cx, cy, prob, threshold, max_iters, _ptr(E),
+                                         ctypes.byref(nsol), _ptr(mask), ctypes.byref(inl)), "hv_find_essential")
+        return np.ascontiguousarray(E.reshape(10, 3, 3)[:nsol.value].transpose(0, 2, 1)), mask[:n]
+
+    def find_essential_device(self, d_xy1, d_xy2, d_E, d_nsol, d_mask, d_inliers, fx, fy, cx, cy, prob=0.999, threshold=1.0,
+                              max_iters=1000, d_status=None, n=None):
+        """hv_find_essential_device on CUDA tensors (see essential_job for the buffers); asynchronous on the context's stream."""
+        j = essential_job(d_xy1, d_xy2, d_E, d_nsol, d_mask, d_inliers, fx, fy, cx, cy, d_status, n)
+        check(self.lib.hv_find_essential_device(self.h, j.d_xy1, j.d_xy2, j.d_status, j.n, fx, fy, cx, cy, prob, threshold, max_iters,
+                                                j.d_E, j.d_nsol, j.d_mask, j.d_inliers), "hv_find_essential_device")
+
+    def find_essential_batch_device(self, jobs, prob=0.999, threshold=1.0, max_iters=1000):
+        """hv_find_essential_batch_device: every job (see essential_job) in one launch; asynchronous."""
+        J = (EssentialJob * len(jobs))(*jobs)
+        check(self.lib.hv_find_essential_batch_device(self.h, J, len(jobs), prob, threshold, max_iters), "hv_find_essential_batch_device")
+
     def lk_track_device(self, prev, nxt, d_prev, d_next, d_status, d_ts, n, use_initial, max_iter=20, eps=0.03, min_eig=1e-3):
         check(self.lib.hv_lk_track_device(self.h, prev.h, nxt.h, _ptr(d_prev), _ptr(d_next), _ptr(d_status), _ptr(d_ts), n,
                                           1 if use_initial else 0, max_iter, eps, min_eig), "hv_lk_track_device")
@@ -456,6 +504,20 @@ def good_features_job(pyr, d_xy, d_count, max_corners, d_response=None, d_mask=N
         _check_cuda_buffer(t)
     mp, ms = _mask_tensor(d_mask, pyr)
     return GoodFeaturesJob(pyr.h.value, max_corners, mp, ms, _ptr(d_xy), _ptr(d_response), d_xy.numel() // 2, _ptr(d_count))
+
+
+def essential_job(d_xy1, d_xy2, d_E, d_nsol, d_mask, d_inliers, fx, fy, cx, cy, d_status=None, n=None):
+    """An EssentialJob on contiguous CUDA tensors: d_xy1, d_xy2 (capacity, 2) float32, d_status (capacity,) uint8 or None, d_E (90,) or
+    (10, 3, 3) float64 (column-major slots), d_nsol and d_inliers (1,) int32, d_mask (capacity,) uint8; n: the first n points (all).
+    The tensors must outlive the call that uses the job."""
+    for t, size in ((d_xy1, 4), (d_xy2, 4), (d_E, 8), (d_nsol, 4), (d_mask, 1), (d_inliers, 4)) + (() if d_status is None else ((d_status, 1),)):
+        if not t.is_cuda or not t.is_contiguous() or t.element_size() != size:
+            raise ValueError("essential_job: every buffer must be a contiguous CUDA tensor of the documented dtype")
+    cap = d_xy1.numel() // 2
+    n = cap if n is None else n
+    if d_xy2.numel() // 2 < n or d_mask.numel() < n or d_E.numel() < 90 or (d_status is not None and d_status.numel() < n) or n > cap:
+        raise ValueError("essential_job: a buffer is smaller than n points (or E smaller than 90 doubles)")
+    return EssentialJob(_ptr(d_xy1), _ptr(d_xy2), _ptr(d_status), n, fx, fy, cx, cy, _ptr(d_E), _ptr(d_nsol), _ptr(d_mask), _ptr(d_inliers))
 
 
 def _dense_rows(img):

@@ -79,6 +79,7 @@ int hv_ctx_destroy(hv_ctx* c)
     if (c->d_selectScratch) cudaFree(c->d_selectScratch);
     if (c->d_fastScratch) cudaFree(c->d_fastScratch);
     if (c->d_gfScratch) cudaFree(c->d_gfScratch);
+    if (c->d_essScratch) cudaFree(c->d_essScratch);
     if (c->d_ekfStage) cudaFree(c->d_ekfStage);
     for (int i = 0; i < HV_EKF_STAGES; i++) {
         if (c->h_ekfStage[i]) cudaFreeHost(c->h_ekfStage[i]);
@@ -1028,6 +1029,145 @@ int hv_good_features_batch_device(hv_ctx* c, const hv_good_features_job* jobs, i
     if (rc != HV_OK) return rc;
     HV_CUDA(hv_launch_good_features_batch(b, njobs, c->stream));
     c->launches += 3;
+    return HV_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ essential-matrix RANSAC (N3)
+// The parameters of the batch: refused as cv::findEssentialMat 4.13 refuses them (prob outside (0, 1), NaN included), or as the device
+// cannot run them (more than HV_ESSENTIAL_MAX_ITERS iterations; maxIters <= 0 runs one, as OpenCV does).
+static int ess_params(const char* who, double prob, int maxIters)
+{
+    if (!(prob > 0.0 && prob < 1.0)) { hv_set_error("%s: prob %g outside (0, 1)", who, prob); return HV_ERR_INVALID; }
+    if (maxIters > HV_ESSENTIAL_MAX_ITERS) {
+        hv_set_error("%s: max_iters %d above %d", who, maxIters, HV_ESSENTIAL_MAX_ITERS);
+        return HV_ERR_UNSUPPORTED;
+    }
+    return HV_OK;
+}
+
+// Checks one job and fills everything but the scratch.
+static int ess_args(const char* who, const float* xy1, const float* xy2, const uint8_t* status, int n, double fx, double fy, double cx,
+                    double cy, double* E, int* nsol, uint8_t* mask, int* inliers, EssentialArgs& a)
+{
+    if (!E || !nsol || !inliers) { hv_set_error("%s: NULL E, nsol or inliers", who); return HV_ERR_INVALID; }
+    if (n < 0) { hv_set_error("%s: n = %d", who, n); return HV_ERR_INVALID; }
+    if (n > 0 && (!xy1 || !xy2 || !mask)) { hv_set_error("%s: NULL xy1, xy2 or mask", who); return HV_ERR_INVALID; }
+    if (n > HV_ESSENTIAL_MAX_POINTS) { hv_set_error("%s: %d points (at most %d)", who, n, HV_ESSENTIAL_MAX_POINTS); return HV_ERR_UNSUPPORTED; }
+    if (!std::isfinite(fx) || !std::isfinite(fy) || !std::isfinite(cx) || !std::isfinite(cy) || fx == 0.0 || fy == 0.0 || fx + fy == 0.0) {
+        hv_set_error("%s: intrinsics (%g, %g, %g, %g) not finite or a zero focal length", who, fx, fy, cx, cy);
+        return HV_ERR_UNSUPPORTED;
+    }
+    memset(&a, 0, sizeof(a));
+    a.xy1 = (const float2*)xy1; a.xy2 = (const float2*)xy2; a.status = status; a.n = n;
+    a.fx = fx; a.fy = fy; a.cx = cx; a.cy = cy;
+    a.E = E; a.nsol = nsol; a.mask = mask; a.inliers = inliers;
+    return HV_OK;
+}
+
+// points the jobs' normalised points and indices into the context's scratch, grown (after the work that may still read it) as needed
+static int ess_scratch(hv_ctx* c, EssentialArgs* jobs, int njobs)
+{
+    size_t total = 0;
+    for (int j = 0; j < njobs; j++) total += align_up(32 * (size_t)jobs[j].n, 256) + align_up(4 * (size_t)jobs[j].n, 256);
+    if (total > c->essScratchBytes) {
+        if (c->d_essScratch) { HV_CUDA(cudaStreamSynchronize(c->stream)); cudaFree(c->d_essScratch); }
+        c->d_essScratch = nullptr; c->essScratchBytes = 0;
+        size_t cap = 1 << 16; while (cap < total) cap *= 2;
+        HV_CUDA(cudaMalloc(&c->d_essScratch, cap));
+        c->essScratchBytes = cap;
+    }
+    uint8_t* p = (uint8_t*)c->d_essScratch;
+    for (int j = 0; j < njobs; j++) {
+        jobs[j].q = (double*)p; p += align_up(32 * (size_t)jobs[j].n, 256);
+        jobs[j].idx = (int*)p; p += align_up(4 * (size_t)jobs[j].n, 256);
+    }
+    return HV_OK;
+}
+
+int hv_find_essential_device(hv_ctx* c, const float* dXY1, const float* dXY2, const uint8_t* dStatus, int n, double fx, double fy,
+                             double cx, double cy, double prob, double threshold, int maxIters, double* dE, int* dNsol, uint8_t* dMask,
+                             int* dInliers)
+{
+    const char* who = "hv_find_essential_device";
+    if (!c) { hv_set_error("%s: NULL context", who); return HV_ERR_INVALID; }
+    int rc = ess_params(who, prob, maxIters);
+    if (rc != HV_OK) return rc;
+    EssentialBatchArgs b;
+    memset(&b, 0, sizeof(b));
+    rc = ess_args(who, dXY1, dXY2, dStatus, n, fx, fy, cx, cy, dE, dNsol, dMask, dInliers, b.job[0]);
+    if (rc != HV_OK) return rc;
+    b.prob = prob; b.threshold = threshold; b.maxIters = maxIters;
+    HV_CUDA(cudaSetDevice(c->device));
+    rc = ess_scratch(c, b.job, 1);
+    if (rc != HV_OK) return rc;
+    HV_CUDA(hv_launch_essential(b, 1, c->stream));
+    c->launches += 1;
+    return HV_OK;
+}
+
+int hv_find_essential(hv_ctx* c, const float* xy1, const float* xy2, const uint8_t* status, int n, double fx, double fy, double cx,
+                      double cy, double prob, double threshold, int maxIters, double* E, int* nsol, uint8_t* mask, int* inliers)
+{
+    const char* who = "hv_find_essential";
+    if (!c) { hv_set_error("%s: NULL context", who); return HV_ERR_INVALID; }
+    int rc = ess_params(who, prob, maxIters);
+    if (rc != HV_OK) return rc;
+    EssentialBatchArgs b;
+    memset(&b, 0, sizeof(b));
+    rc = ess_args(who, xy1, xy2, status, n, fx, fy, cx, cy, E, nsol, mask, inliers, b.job[0]);
+    if (rc != HV_OK) return rc;
+    b.prob = prob; b.threshold = threshold; b.maxIters = maxIters;
+    HV_CUDA(cudaSetDevice(c->device));
+    rc = ess_scratch(c, b.job, 1);
+    if (rc != HV_OK) return rc;
+    // staging block: [E 80 doubles | nsol, inliers | mask n] back to the host, [xy1 8n | xy2 8n | status n] to the device
+    const size_t oMask = 8 * 90 + 16, oXY1 = align_up(oMask + (size_t)n, 16);
+    const size_t oXY2 = oXY1 + 8 * (size_t)n, oSt = oXY2 + 8 * (size_t)n, total = oSt + (status ? (size_t)n : 0);
+    rc = hv_ctx_reserve_stage(c, total);
+    if (rc != HV_OK) return rc;
+    uint8_t* hs = (uint8_t*)c->h_stage; uint8_t* ds = (uint8_t*)c->d_stage;
+    if (n > 0) {
+        memcpy(hs + oXY1, xy1, 8 * (size_t)n);
+        memcpy(hs + oXY2, xy2, 8 * (size_t)n);
+        if (status) memcpy(hs + oSt, status, (size_t)n);
+    }
+    if (total > oXY1) HV_CUDA(cudaMemcpyAsync(ds + oXY1, hs + oXY1, total - oXY1, cudaMemcpyHostToDevice, c->stream));
+    EssentialArgs& a = b.job[0];
+    a.xy1 = (const float2*)(ds + oXY1); a.xy2 = (const float2*)(ds + oXY2); a.status = status ? ds + oSt : nullptr;
+    a.E = (double*)ds; a.nsol = (int*)(ds + 8 * 90); a.inliers = (int*)(ds + 8 * 90 + 4); a.mask = ds + oMask;
+    HV_CUDA(hv_launch_essential(b, 1, c->stream));
+    c->launches += 1;
+    HV_CUDA(cudaMemcpyAsync(hs, ds, oMask + (size_t)n, cudaMemcpyDeviceToHost, c->stream));
+    HV_CUDA(cudaStreamSynchronize(c->stream));
+    memcpy(E, hs, 8 * 90);
+    memcpy(nsol, hs + 8 * 90, sizeof(int));
+    memcpy(inliers, hs + 8 * 90 + 4, sizeof(int));
+    if (n > 0) memcpy(mask, hs + oMask, (size_t)n);
+    return HV_OK;
+}
+
+int hv_find_essential_batch_device(hv_ctx* c, const hv_essential_job* jobs, int njobs, double prob, double threshold, int maxIters)
+{
+    const char* who = "hv_find_essential_batch_device";
+    if (!c || !jobs) { hv_set_error("%s: NULL context or jobs", who); return HV_ERR_INVALID; }
+    if (njobs < 1 || njobs > HV_ESSENTIAL_BATCH_MAX) { hv_set_error("%s: %d jobs (1..%d per call)", who, njobs, HV_ESSENTIAL_BATCH_MAX); return HV_ERR_INVALID; }
+    int rc = ess_params(who, prob, maxIters);
+    if (rc != HV_OK) return rc;
+    EssentialBatchArgs b;
+    memset(&b, 0, sizeof(b));
+    for (int j = 0; j < njobs; j++) {
+        const hv_essential_job& J = jobs[j];
+        char w[64];
+        snprintf(w, sizeof(w), "%s job %d", who, j);
+        rc = ess_args(w, J.d_xy1, J.d_xy2, J.d_status, J.n, J.fx, J.fy, J.cx, J.cy, J.d_E, J.d_nsol, J.d_mask, J.d_inliers, b.job[j]);
+        if (rc != HV_OK) return rc;
+    }
+    b.prob = prob; b.threshold = threshold; b.maxIters = maxIters;
+    HV_CUDA(cudaSetDevice(c->device));
+    rc = ess_scratch(c, b.job, njobs);
+    if (rc != HV_OK) return rc;
+    HV_CUDA(hv_launch_essential(b, njobs, c->stream));
+    c->launches += 1;
     return HV_OK;
 }
 

@@ -31,6 +31,7 @@ struct hv_ctx {
     float* d_selectScratch = nullptr; size_t selectScratchBytes = 0;     // hv_gftt_corners: key points and previous corners (device)
     void* d_fastScratch = nullptr; size_t fastScratchBytes = 0;          // hv_fast_detect*: keypoint masks and tile counts (device)
     void* d_gfScratch = nullptr; size_t gfScratchBytes = 0;              // hv_good_features*: per-job words, response maps, keys, grids
+    void* d_essScratch = nullptr; size_t essScratchBytes = 0;            // hv_find_essential*: per-job normalised points and indices
     unsigned* d_done = nullptr;        // completion counter of the polled launches (device)
     unsigned doneCount = 0, seq = 0;   // host mirror of the counter / sequence number of the last polled launch
     // EKF group staging (hv_ekf_group_run_device): a call's argument blocks reach the device in one copy out of a ring of pinned blocks

@@ -222,6 +222,28 @@ struct GoodFeaturesBatchArgs {
 static_assert(sizeof(GoodFeaturesBatchArgs) <= HV_KERNEL_PARAM_MAX, "good-features batch arguments exceed the kernel-parameter space");
 cudaError_t hv_launch_good_features_batch(const GoodFeaturesBatchArgs& b, int njobs, cudaStream_t stream);
 
+// ---- essential-matrix RANSAC (essential.cu): cv::findEssentialMat(..., RANSAC, prob, threshold, maxIters) on the used points
+#define HV_ESSENTIAL_BATCH_MAX 64
+#define HV_ESSENTIAL_MAX_POINTS 4096
+#define HV_ESSENTIAL_MAX_ITERS 4096
+struct EssentialArgs {
+    const float2* xy1; const float2* xy2;
+    const uint8_t* status;            // NULL: every point is used
+    int n;
+    double fx, fy, cx, cy;
+    double* E;                        // 10 column-major 3 x 3 slots
+    int* nsol; uint8_t* mask; int* inliers;
+    double* q;                        // scratch: n normalised used points (x1, y1, x2, y2), 32-byte aligned
+    int* idx;                         // scratch: their original indices
+};
+struct EssentialBatchArgs {
+    EssentialArgs job[HV_ESSENTIAL_BATCH_MAX];
+    double prob, threshold;
+    int maxIters;
+};
+static_assert(sizeof(EssentialBatchArgs) <= HV_KERNEL_PARAM_MAX, "essential batch arguments exceed the kernel-parameter space");
+cudaError_t hv_launch_essential(const EssentialBatchArgs& b, int njobs, cudaStream_t stream);     // one launch, one CTA per job
+
 // ---- frame ingest (ingest.cu)
 #define HV_REMAP_INVALID (-32768)
 struct HvRemapEntry { short x0, y0; float xfrac, yfrac; };      // 12 bytes per output pixel (hv_remap_entry of the C ABI)

@@ -270,6 +270,48 @@ typedef struct hv_good_features_job {
 int hv_good_features_batch_device(hv_ctx* ctx, const hv_good_features_job* jobs, int njobs, int block_size, double quality_level,
                                   double min_distance);
 
+/* ---------------------------------------------------------------- essential-matrix RANSAC (SURVEY.md 8(f) N3) -- */
+/* cv::findEssentialMat(xy1[used], xy2[used], K, RANSAC, prob, threshold, max_iters, mask) (OCV/calib3d/src/five-point.cpp, ptsetreg.cpp):
+ * the five-point RANSAC that the reference's RANSAC-5 stage is built on (how its modified copy differs from OpenCV is not restated here),
+ * K = [[fx, 0, cx], [0, fy, cy], [0, 0, 1]]. The used points are those with status != 0 (all n when status is NULL), in index order; m is
+ * their count. RANSAC replays OpenCV's: cv::RNG seeded with ~0 draws the subsets, a count above max(best, 4) wins, the iteration bound
+ * shrinks through RANSACUpdateNumIters, an error is an inlier when (float)Sampson <= (float)((threshold / ((fx + fy) / 2))^2).
+ * The five-point solver is this library's own (DESIGN.md 4.11): the same essential matrices as OpenCV's up to rounding, the solutions
+ * of one subset in ascending order of their hidden variable. Where two solutions of one subset reach the same winning inlier count, OpenCV
+ * keeps the first in its own root order, which is not restated, so its E (rarely its mask) can then be the other one.
+ *   xy1, xy2  n x (x, y) float32: the correspondences (the layout the LK calls write)
+ *   status    n x u8 or NULL; LK's status over a padded capacity (HV_CORNER_NONE slots report 0) can be passed as it is
+ *   E         10 column-major fp64 3 x 3 slots: m < 5: none; m == 5: every solution of the five points (nsol <= 10);
+ *             m > 5: the best one (nsol = 1), or none (nsol = 0) where OpenCV returns none. Slots [nsol, 10) are 0.
+ *   mask      n x u8: 1 for the used points that are inliers of the result (m == 5: the five points when nsol > 0), 0 elsewhere
+ *   inliers   the number of ones in mask
+ * max_iters <= 0 runs one iteration, as OpenCV does; threshold may be any value OpenCV accepts (it is squared; NaN finds no inlier).
+ * Errors, before anything is launched (buffers and the context's launch count untouched): HV_ERR_INVALID for a NULL context / E / nsol /
+ * inliers, a NULL xy1 / xy2 / mask with n > 0, n < 0, or prob outside (0, 1) or NaN (what cv::findEssentialMat 4.13 refuses);
+ * HV_ERR_UNSUPPORTED for n above HV_ESSENTIAL_MAX_POINTS, max_iters above HV_ESSENTIAL_MAX_ITERS, and intrinsics that are not finite or
+ * have a zero focal length (OpenCV accepts them and returns NaN-laden results).
+ * Every call is one launch (ctx's launch count + 1) whatever the data holds. The normalised points and their indices live in scratch
+ * memory of the context (36 bytes per point), which only grows. */
+#define HV_ESSENTIAL_MAX_POINTS 4096
+#define HV_ESSENTIAL_MAX_ITERS 4096
+int hv_find_essential(hv_ctx* ctx, const float* xy1, const float* xy2, const uint8_t* status, int n, double fx, double fy, double cx,
+                      double cy, double prob, double threshold, int max_iters, double* E, int* nsol, uint8_t* mask, int* inliers); /* host, synchronises */
+int hv_find_essential_device(hv_ctx* ctx, const float* d_xy1, const float* d_xy2, const uint8_t* d_status, int n, double fx, double fy,
+                             double cx, double cy, double prob, double threshold, int max_iters, double* d_E, int* d_nsol, uint8_t* d_mask,
+                             int* d_inliers);                                                                      /* device, asynchronous */
+/* hv_find_essential_device for up to HV_ESSENTIAL_BATCH_MAX jobs (one per session sharing the context) in the one launch of one call:
+ * every job's outputs are bit-identical to the per-call function's. Points, status, n, intrinsics and outputs are per job; prob,
+ * threshold and max_iters the batch's. Errors as hv_find_essential_device's for every job, and HV_ERR_INVALID for a NULL jobs array or
+ * njobs outside 1..HV_ESSENTIAL_BATCH_MAX, all before anything is launched. */
+#define HV_ESSENTIAL_BATCH_MAX 64
+typedef struct hv_essential_job {
+    const float* d_xy1; const float* d_xy2; const uint8_t* d_status;
+    int n;
+    double fx, fy, cx, cy;
+    double* d_E; int* d_nsol; uint8_t* d_mask; int* d_inliers;
+} hv_essential_job;
+int hv_find_essential_batch_device(hv_ctx* ctx, const hv_essential_job* jobs, int njobs, double prob, double threshold, int max_iters);
+
 /* ---------------------------------------------------------------- frame ingest (SURVEY.md 8(f) N4) -------- */
 /* Device part of tracker::Image::Factory::build / buildStereo (src/tracker/image.cpp:243-308): colour -> gray
  * (accelerated-arrays pixelwiseAffine, image.cpp:360-366) and undistortion / rectification (UndistorterImplementation::undistort,
