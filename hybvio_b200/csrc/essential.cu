@@ -141,11 +141,59 @@ __device__ __noinline__ static void ess_constraint(const double (*N)[9], int e, 
     }
 }
 
-__device__ static void ess_pmul(const double* a, int na, const double* b, int nb, double* out)
+// double-double arithmetic (hi + lo), operation for operation as the oracle's dd_* (fma only where written out): the elimination, the
+// determinant and the determinant's sign in the root brackets lose digits to cancellation in double
+struct EssDD { double hi, lo; };
+
+__device__ __forceinline__ EssDD ess_dd_fast(double s, double e)
 {
-    for (int k = 0; k < na + nb - 1; k++) out[k] = 0.0;
+    const double h = s + e;
+    return EssDD{h, e - (h - s)};
+}
+
+__device__ __forceinline__ EssDD ess_dd_two_sum(double a, double b)
+{
+    const double s = a + b, bb = s - a;
+    return EssDD{s, (a - (s - bb)) + (b - bb)};
+}
+
+__device__ __forceinline__ EssDD ess_dd_add(EssDD a, EssDD b)
+{
+    EssDD s = ess_dd_two_sum(a.hi, b.hi);
+    const EssDD t = ess_dd_two_sum(a.lo, b.lo);
+    s = ess_dd_fast(s.hi, s.lo + t.hi);
+    return ess_dd_fast(s.hi, s.lo + t.lo);
+}
+
+__device__ __forceinline__ EssDD ess_dd_sub(EssDD a, EssDD b) { return ess_dd_add(a, EssDD{-b.hi, -b.lo}); }
+
+__device__ __forceinline__ EssDD ess_dd_mul(EssDD a, EssDD b)
+{
+    const double p = a.hi * b.hi;
+    const double e = fma(a.hi, b.hi, -p) + (a.hi * b.lo + a.lo * b.hi);
+    return ess_dd_fast(p, e);
+}
+
+__device__ __forceinline__ EssDD ess_dd_mul_d(EssDD a, double x)
+{
+    const double p = a.hi * x;
+    return ess_dd_fast(p, fma(a.hi, x, -p) + a.lo * x);
+}
+
+__device__ __forceinline__ EssDD ess_dd_div(EssDD a, EssDD b)
+{
+    const double q1 = a.hi / b.hi;
+    const EssDD r = ess_dd_sub(a, ess_dd_mul(b, EssDD{q1, 0.0}));
+    return ess_dd_fast(q1, r.hi / b.hi);
+}
+
+// coefficient k of the product of the polynomials a (na coefficients) and b (nb), summed in ascending order of a's index
+__device__ static EssDD ess_dd_conv(const EssDD* a, int na, const EssDD* b, int nb, int k)
+{
+    EssDD s{0.0, 0.0};
     for (int i = 0; i < na; i++)
-        for (int j = 0; j < nb; j++) out[i + j] = out[i + j] + a[i] * b[j];
+        if (k - i >= 0 && k - i < nb) s = ess_dd_add(s, ess_dd_mul(a[i], b[k - i]));
+    return s;
 }
 
 __device__ static int ess_sgn(double v) { return (v > 0.0) - (v < 0.0); }
@@ -196,12 +244,40 @@ __device__ __noinline__ int ess_interval_root(const double* g, double lo, double
     return 1;
 }
 
+// the interval (lo, hi] of the determinant itself (double-double coefficients c, degree d, shared memory), as ess_interval_root<D>
+// with the sign of its value in double-double (Horner's rule, ess_dd_mul_d then ess_dd_add per coefficient)
+__device__ static double ess_horner_dd(const EssDD* c, int d, double x)
+{
+    EssDD s = c[d];
+    for (int i = d - 1; i >= 0; i--) s = ess_dd_add(ess_dd_mul_d(s, x), c[i]);
+    return s.hi;
+}
+
+__device__ __noinline__ int ess_interval_root_dd(const EssDD* c, int d, double lo, double hi, double* root)
+{
+    const int slo = ess_sgn(ess_horner_dd(c, d, lo)), shi = ess_sgn(ess_horner_dd(c, d, hi));
+    if (slo != 0 && shi == 0) { *root = hi; return 1; }
+    if (slo == 0 || shi == 0 || slo == shi) return 0;
+    long long kl = ess_okey(lo), kh = ess_okey(hi);
+    for (int it = 0; it < ESS_BISECT; it++) {
+        const unsigned long long span = (unsigned long long)kh - (unsigned long long)kl;
+        if (span <= 1) continue;
+        const long long km = kl + (long long)(span >> 1);
+        if (ess_sgn(ess_horner_dd(c, d, ess_ofrom(km))) == slo) kl = km; else kh = km;
+    }
+    *root = ess_ofrom(kh);
+    return 1;
+}
+
 // per-warp solver workspace (shared memory)
 struct EssWarp {
-    double M[10][20], M0[10][20];     // the coefficient matrix during elimination, and as formed
+    EssDD M[10][20];                  // the coefficient matrix during elimination (double-double)
+    double M0[10][20];                // as formed
     double N[4][9];                   // null-space basis X, Y, Z, W
-    double P[3][4], Qp[3][4], R[3][5];
-    double poly[11];
+    EssDD Pd[3][4], Qd[3][4], Rd[3][5], m0[8], m1[8], m2[7];
+    EssDD pdd[11];                    // the determinant
+    double P[3][4], Qp[3][4], R[3][5];  // Pd, Qd, Rd rounded to double (the recovery)
+    double poly[11];                  // pdd rounded to double (the derivatives)
     double der[11][11];               // der[d]: the derivative of degree d of the determinant
     double crit[10];                  // the real roots of the previous level, ascending
 };
@@ -234,7 +310,8 @@ __device__ static int ess_real_roots(EssWarp& w, int lane)
         if (lane <= ncrit) {
             const double lo = lane == 0 ? -R : w.crit[lane - 1], hi = lane == ncrit ? R : w.crit[lane];
             const double* g = w.der[d];
-            switch (d) {
+            if (d == D) has = ess_interval_root_dd(w.pdd, D, lo, hi, &root);
+            else switch (d) {
             case 1: has = ess_interval_root<1>(g, lo, hi, &root); break;
             case 2: has = ess_interval_root<2>(g, lo, hi, &root); break;
             case 3: has = ess_interval_root<3>(g, lo, hi, &root); break;
@@ -370,8 +447,8 @@ __device__ __noinline__ static int ess_recover(const EssWarp& w, double z, doubl
 }
 
 // every essential matrix (row-major, unit Frobenius norm) of five normalised correspondences q = (x1, y1, x2, y2) into sols, in
-// ascending order of their roots. Every lane of the warp calls it: lane 0 forms the null space and the determinant, lanes 0-9 the
-// constraints, lanes 0-19 one column each of the elimination, lane k the roots in interval k of each level and the matrix of root k.
+// ascending order of their roots. Every lane of the warp calls it: lane 0 forms the null space, lanes 0-9 the constraints, lanes 0-19
+// one column each of the elimination, lanes 0-10 the determinant, lane k the roots in interval k of each level and the matrix of root k.
 // Returns their number.
 __device__ static int ess_solve5(const double* q, double (*sols)[9], EssWarp& w, int lane)
 {
@@ -413,46 +490,57 @@ __device__ static int ess_solve5(const double* q, double (*sols)[9], EssWarp& w,
     }
     __syncwarp();
     if (lane < 10) {
-        ess_constraint(w.N, lane, w.M[lane]);
-        for (int j = 0; j < 20; j++) w.M0[lane][j] = w.M[lane][j];
+        ess_constraint(w.N, lane, w.M0[lane]);
+        for (int j = 0; j < 20; j++) w.M[lane][j] = EssDD{w.M0[lane][j], 0.0};
     }
     __syncwarp();
-    // Gauss-Jordan with partial pivoting, lane j < 20 owning column j
+    // Gauss-Jordan with partial pivoting in double-double, lane j < 20 owning column j
     for (int k = 0; k < 10; k++) {
         int p = k;
         for (int r = k + 1; r < 10; r++)
-            if (fabs(w.M[r][k]) > fabs(w.M[p][k])) p = r;
-        double f[10];
+            if (fabs(w.M[r][k].hi) > fabs(w.M[p][k].hi)) p = r;
+        EssDD f[10];
         for (int r = 0; r < 10; r++) f[r] = w.M[r == k ? p : r == p ? k : r][k];
-        const double piv = f[k];
+        const EssDD piv = f[k];
         __syncwarp();
-        if (piv == 0.0 || piv != piv) return 0;
+        if (piv.hi == 0.0 || piv.hi != piv.hi) return 0;
         if (lane < 20) {
             const int j = lane;
-            if (p != k) { const double t = w.M[k][j]; w.M[k][j] = w.M[p][j]; w.M[p][j] = t; }
-            w.M[k][j] = w.M[k][j] / piv;
+            if (p != k) { const EssDD t = w.M[k][j]; w.M[k][j] = w.M[p][j]; w.M[p][j] = t; }
+            w.M[k][j] = ess_dd_div(w.M[k][j], piv);
             for (int r = 0; r < 10; r++)
-                if (r != k) w.M[r][j] = w.M[r][j] - f[r] * w.M[k][j];
+                if (r != k) w.M[r][j] = ess_dd_sub(w.M[r][j], ess_dd_mul(f[r], w.M[k][j]));
         }
         __syncwarp();
     }
+    // the determinant in double-double: lane 0 the 3 x 3 matrix, lanes 0-7 the 2 x 2 minors' coefficients, lanes 0-10 its own
     if (lane == 0) {
         for (int i = 0; i < 3; i++) {
-            const double* e = w.M[4 + 2 * i] + 10;
-            const double* f = w.M[5 + 2 * i] + 10;
-            w.P[i][0] = e[2]; w.P[i][1] = e[1] - f[2]; w.P[i][2] = e[0] - f[1]; w.P[i][3] = -f[0];
-            w.Qp[i][0] = e[5]; w.Qp[i][1] = e[4] - f[5]; w.Qp[i][2] = e[3] - f[4]; w.Qp[i][3] = -f[3];
-            w.R[i][0] = e[9]; w.R[i][1] = e[8] - f[9]; w.R[i][2] = e[7] - f[8]; w.R[i][3] = e[6] - f[7]; w.R[i][4] = -f[6];
+            const EssDD* e = w.M[4 + 2 * i] + 10;
+            const EssDD* f = w.M[5 + 2 * i] + 10;
+            const EssDD z{0.0, 0.0};
+            w.Pd[i][0] = e[2]; w.Pd[i][1] = ess_dd_sub(e[1], f[2]); w.Pd[i][2] = ess_dd_sub(e[0], f[1]); w.Pd[i][3] = ess_dd_sub(z, f[0]);
+            w.Qd[i][0] = e[5]; w.Qd[i][1] = ess_dd_sub(e[4], f[5]); w.Qd[i][2] = ess_dd_sub(e[3], f[4]); w.Qd[i][3] = ess_dd_sub(z, f[3]);
+            w.Rd[i][0] = e[9]; w.Rd[i][1] = ess_dd_sub(e[8], f[9]); w.Rd[i][2] = ess_dd_sub(e[7], f[8]); w.Rd[i][3] = ess_dd_sub(e[6], f[7]);
+            w.Rd[i][4] = ess_dd_sub(z, f[6]);
+            for (int c = 0; c < 4; c++) { w.P[i][c] = w.Pd[i][c].hi; w.Qp[i][c] = w.Qd[i][c].hi; }
+            for (int c = 0; c < 5; c++) w.R[i][c] = w.Rd[i][c].hi;
         }
-        double t1[8], t2[8], m0[8], m1[8], m2[7], d0[11], d1[11], d2[11];
-        ess_pmul(w.Qp[1], 4, w.R[2], 5, t1); ess_pmul(w.Qp[2], 4, w.R[1], 5, t2);
-        for (int k = 0; k < 8; k++) m0[k] = t1[k] - t2[k];
-        ess_pmul(w.P[1], 4, w.R[2], 5, t1); ess_pmul(w.P[2], 4, w.R[1], 5, t2);
-        for (int k = 0; k < 8; k++) m1[k] = t1[k] - t2[k];
-        ess_pmul(w.P[1], 4, w.Qp[2], 4, t1); ess_pmul(w.P[2], 4, w.Qp[1], 4, t2);
-        for (int k = 0; k < 7; k++) m2[k] = t1[k] - t2[k];
-        ess_pmul(w.P[0], 4, m0, 8, d0); ess_pmul(w.Qp[0], 4, m1, 8, d1); ess_pmul(w.R[0], 5, m2, 7, d2);
-        for (int k = 0; k < 11; k++) w.poly[k] = (d0[k] - d1[k]) + d2[k];
+    }
+    __syncwarp();
+    if (lane < 8) {
+        const int k = lane;
+        w.m0[k] = ess_dd_sub(ess_dd_conv(w.Qd[1], 4, w.Rd[2], 5, k), ess_dd_conv(w.Qd[2], 4, w.Rd[1], 5, k));
+        w.m1[k] = ess_dd_sub(ess_dd_conv(w.Pd[1], 4, w.Rd[2], 5, k), ess_dd_conv(w.Pd[2], 4, w.Rd[1], 5, k));
+        if (k < 7) w.m2[k] = ess_dd_sub(ess_dd_conv(w.Pd[1], 4, w.Qd[2], 4, k), ess_dd_conv(w.Pd[2], 4, w.Qd[1], 4, k));
+    }
+    __syncwarp();
+    if (lane < 11) {
+        const int k = lane;
+        const EssDD v = ess_dd_add(ess_dd_sub(ess_dd_conv(w.Pd[0], 4, w.m0, 8, k), ess_dd_conv(w.Qd[0], 4, w.m1, 8, k)),
+                                   ess_dd_conv(w.Rd[0], 5, w.m2, 7, k));
+        w.pdd[k] = v;
+        w.poly[k] = v.hi;
     }
     __syncwarp();
     const int nr = ess_real_roots(w, lane);

@@ -14,15 +14,18 @@
  *   a. Householder QR of the 5 x 9 epipolar matrix Q^T; the last four columns of the orthogonal factor span the null space of Q:
  *      E = x X + y Y + z Z + W;
  *   b. the ten cubic constraints det(E) = 0 and E E^T E - tr(E E^T) E / 2 = 0 in the 20 monomials of x, y, z (Nister's order);
- *   c. Gauss-Jordan elimination with partial pivoting of the 10 x 20 coefficient matrix;
- *   d. the 3 x 3 matrix of polynomials in z (rows <e> - z <f>, <g> - z <h>, <i> - z <j>) and its degree-10 determinant;
+ *   c. Gauss-Jordan elimination with partial pivoting of the 10 x 20 coefficient matrix, in double-double;
+ *   d. the 3 x 3 matrix of polynomials in z (rows <e> - z <f>, <g> - z <h>, <i> - z <j>) and its degree-10 determinant, in
+ *      double-double;
  *   e. the real roots of the determinant by recursion on the derivatives: the real roots of p' split the real line into intervals on
- *      which p is monotonic; an interval whose ends differ in sign holds one root, bracketed by 48 bisection steps on the ordered bit
+ *      which p is monotonic; an interval whose ends differ in sign holds one root (p itself evaluated in double-double, its
+ *      derivatives from its coefficients rounded to double), bracketed by 48 bisection steps on the ordered bit
  *      patterns of doubles (within 2^16 ulps at the end, whatever the root's magnitude): a fixed amount of work for any data;
  *   f. per root, ascending: (x, y, 1) from the largest cross product of two rows of the 3 x 3 matrix (skipped when the unit vector's
- *      last entry is below 1e-10, as OpenCV skips it), (x, y, z) polished by Gauss-Newton steps on the ten constraints, E normalised
+ *      last entry is below 1e-10, as OpenCV skips it), (x, y, z) polished by four Gauss-Newton steps on the ten constraints, E normalised
  *      to unit Frobenius norm.
- * Built with -ffp-contract=off, so no multiply-add is contracted; the kernel is built with --fmad=false.
+ * Built with -ffp-contract=off, so no multiply-add is contracted (the double-double products call fma explicitly); the kernel is built
+ * with --fmad=false.
  */
 #include <float.h>
 #include <math.h>
@@ -108,11 +111,67 @@ static void constraint(const double N[4][9], int e, double* row)
     for (int k = 0; k < 20; k++) row[k] = row[k] - c[k];
 }
 
-static void pmul(const double* a, int na, const double* b, int nb, double* out)
+/* double-double arithmetic (a value hi + lo, |lo| <= ulp(hi) / 2; fma only where written out, for the exact error of a product):
+ * the elimination and the determinant of step d. lose digits to cancellation, and in fp64 a close pair of real roots of the
+ * determinant could turn complex (two solutions lost) or move by 0.5 (solutions that are not essential matrices) */
+typedef struct { double hi, lo; } dd;
+
+static dd dd_fast(double s, double e)
 {
-    for (int k = 0; k < na + nb - 1; k++) out[k] = 0.0;
+    const double h = s + e;
+    const dd r = {h, e - (h - s)};
+    return r;
+}
+
+static dd dd_two_sum(double a, double b)
+{
+    const double s = a + b, bb = s - a;
+    const dd r = {s, (a - (s - bb)) + (b - bb)};
+    return r;
+}
+
+static dd dd_add(dd a, dd b)
+{
+    dd s = dd_two_sum(a.hi, b.hi);
+    const dd t = dd_two_sum(a.lo, b.lo);
+    s = dd_fast(s.hi, s.lo + t.hi);
+    return dd_fast(s.hi, s.lo + t.lo);
+}
+
+static dd dd_sub(dd a, dd b)
+{
+    const dd nb = {-b.hi, -b.lo};
+    return dd_add(a, nb);
+}
+
+static dd dd_mul(dd a, dd b)
+{
+    const double p = a.hi * b.hi;
+    const double e = fma(a.hi, b.hi, -p) + (a.hi * b.lo + a.lo * b.hi);
+    return dd_fast(p, e);
+}
+
+static dd dd_mul_d(dd a, double x)
+{
+    const double p = a.hi * x;
+    return dd_fast(p, fma(a.hi, x, -p) + a.lo * x);
+}
+
+static dd dd_div(dd a, dd b)
+{
+    const double q1 = a.hi / b.hi;
+    const dd q = {q1, 0.0};
+    const dd r = dd_sub(a, dd_mul(b, q));
+    return dd_fast(q1, r.hi / b.hi);
+}
+
+/* coefficient k of the product of the polynomials a (na coefficients) and b (nb), summed in ascending order of a's index */
+static dd dd_conv(const dd* a, int na, const dd* b, int nb, int k)
+{
+    dd s = {0.0, 0.0};
     for (int i = 0; i < na; i++)
-        for (int j = 0; j < nb; j++) out[i + j] = out[i + j] + a[i] * b[j];
+        if (k - i >= 0 && k - i < nb) s = dd_add(s, dd_mul(a[i], b[k - i]));
+    return s;
 }
 
 static double horner(const double* c, int d, double x)
@@ -120,6 +179,15 @@ static double horner(const double* c, int d, double x)
     double s = c[d];
     for (int i = d - 1; i >= 0; i--) s = s * x + c[i];
     return s;
+}
+
+/* Horner's rule in double-double for the determinant itself: next to a close pair of real roots its value is far below the rounding
+ * of its terms in double */
+static double horner_dd(const dd* c, int d, double x)
+{
+    dd s = c[d];
+    for (int i = d - 1; i >= 0; i--) s = dd_add(dd_mul_d(s, x), c[i]);
+    return s.hi;
 }
 
 static int sgn(double v) { return (v > 0.0) - (v < 0.0); }
@@ -143,21 +211,26 @@ static double ofrom(int64_t k)
 /* the root of the degree-d polynomial c in (lo, hi], where its sign at lo is slo and differs at hi: ESS_BISECT steps leave at most 2^16
  * ulps of the root (about 1.5e-11 of its magnitude), which the Gauss-Newton polish takes to full precision */
 #define ESS_BISECT 48
-static double bisect(const double* c, int d, double lo, double hi, int slo)
+static double eval(const double* c, const dd* cd, int d, double x) { return cd ? horner_dd(cd, d, x) : horner(c, d, x); }
+
+static double bisect(const double* c, const dd* cd, int d, double lo, double hi, int slo)
 {
     int64_t kl = okey(lo), kh = okey(hi);
     for (int it = 0; it < ESS_BISECT; it++) {
         const uint64_t span = (uint64_t)kh - (uint64_t)kl;
         if (span <= 1) continue;
         const int64_t km = kl + (int64_t)(span >> 1);
-        if (sgn(horner(c, d, ofrom(km))) == slo) kl = km; else kh = km;
+        if (sgn(eval(c, cd, d, ofrom(km))) == slo) kl = km; else kh = km;
     }
     return ofrom(kh);
 }
 
-/* the real roots of the polynomial p (ascending coefficients, degree <= 10), ascending; returns their number */
-static int real_roots(const double* p, double* roots)
+/* the real roots of the polynomial pd (double-double, ascending coefficients, degree <= 10), ascending; returns their number. The
+ * derivatives are formed from the coefficients rounded to double; the last level evaluates pd itself in double-double. */
+static int real_roots(const dd* pd, double* roots)
 {
+    double p[11];
+    for (int i = 0; i <= 10; i++) p[i] = pd[i].hi;
     int D = 10;
     while (D > 0 && p[D] == 0.0) D--;
     if (D < 1) return 0;
@@ -178,8 +251,9 @@ static int real_roots(const double* p, double* roots)
         ncur = 0;
         for (int k = 0; k <= ncrit; k++) {
             const double lo = k == 0 ? -R : crit[k - 1], hi = k == ncrit ? R : crit[k];
-            const int slo = sgn(horner(der[d], d, lo)), shi = sgn(horner(der[d], d, hi));
-            if (slo != 0 && shi != 0 && slo != shi) cur[ncur++] = bisect(der[d], d, lo, hi, slo);
+            const dd* cd = d == D ? pd : NULL;
+            const int slo = sgn(eval(der[d], cd, d, lo)), shi = sgn(eval(der[d], cd, d, hi));
+            if (slo != 0 && shi != 0 && slo != shi) cur[ncur++] = bisect(der[d], cd, d, lo, hi, slo);
             else if (slo != 0 && shi == 0) cur[ncur++] = hi;
         }
         for (int k = 0; k < ncur; k++) crit[k] = cur[k];
@@ -201,8 +275,8 @@ static void monomials(double x, double y, double z, double* v, double* dx, doubl
 }
 
 /* ESS_POLISH Gauss-Newton steps on the ten constraints M0 (the coefficient matrix before elimination) from (x, y, z); 0 when the
- * normal equations are singular. The degree-10 determinant loses digits to cancellation (its roots alone leave residuals up to 1e-7 in
- * the constraints); four steps bring every solution of the 2000 configurations of tests/test_oracle_essential.py below 1e-12. */
+ * normal equations are singular. The roots of the determinant leave residuals in the constraints because its coefficients are rounded
+ * to double for the derivatives and the recovery; four steps bring the solutions of tests/test_essential_ref.py within their bound. */
 #define ESS_POLISH 4
 static int polish(const double M0[10][20], double* px, double* py, double* pz)
 {
@@ -277,43 +351,49 @@ int orc_ess_solve5(const double* q, double* sols)
             for (int i = k; i < 9; i++) N[c][i] = N[c][i] - f * V[k][i];
         }
     }
-    /* b. - c. */
-    double M[10][20], M0[10][20];
-    for (int e = 0; e < 10; e++) constraint(N, e, M[e]);
-    memcpy(M0, M, sizeof(M0));
+    /* b. - c. (the elimination in double-double) */
+    double M0[10][20];
+    dd M[10][20];
+    for (int e = 0; e < 10; e++) constraint(N, e, M0[e]);
+    for (int e = 0; e < 10; e++)
+        for (int j = 0; j < 20; j++) { M[e][j].hi = M0[e][j]; M[e][j].lo = 0.0; }
     for (int k = 0; k < 10; k++) {
         int p = k;
         for (int r = k + 1; r < 10; r++)
-            if (fabs(M[r][k]) > fabs(M[p][k])) p = r;
+            if (fabs(M[r][k].hi) > fabs(M[p][k].hi)) p = r;
         if (p != k)
-            for (int j = 0; j < 20; j++) { const double t = M[k][j]; M[k][j] = M[p][j]; M[p][j] = t; }
-        const double piv = M[k][k];
-        if (piv == 0.0 || piv != piv) return 0;
-        double f[10];
+            for (int j = 0; j < 20; j++) { const dd t = M[k][j]; M[k][j] = M[p][j]; M[p][j] = t; }
+        const dd piv = M[k][k];
+        if (piv.hi == 0.0 || piv.hi != piv.hi) return 0;
+        dd f[10];
         for (int r = 0; r < 10; r++) f[r] = M[r][k];
-        for (int j = 0; j < 20; j++) M[k][j] = M[k][j] / piv;
+        for (int j = 0; j < 20; j++) M[k][j] = dd_div(M[k][j], piv);
         for (int r = 0; r < 10; r++)
             if (r != k)
-                for (int j = 0; j < 20; j++) M[r][j] = M[r][j] - f[r] * M[k][j];
+                for (int j = 0; j < 20; j++) M[r][j] = dd_sub(M[r][j], dd_mul(f[r], M[k][j]));
     }
-    /* d. */
+    /* d. (double-double; P, Qp and R rounded to double for step f.) */
+    dd Pd[3][4], Qd[3][4], Rd[3][5];
     double P[3][4], Qp[3][4], R[3][5];
     for (int i = 0; i < 3; i++) {
-        const double* e = M[4 + 2 * i] + 10;
-        const double* f = M[5 + 2 * i] + 10;
-        P[i][0] = e[2]; P[i][1] = e[1] - f[2]; P[i][2] = e[0] - f[1]; P[i][3] = -f[0];
-        Qp[i][0] = e[5]; Qp[i][1] = e[4] - f[5]; Qp[i][2] = e[3] - f[4]; Qp[i][3] = -f[3];
-        R[i][0] = e[9]; R[i][1] = e[8] - f[9]; R[i][2] = e[7] - f[8]; R[i][3] = e[6] - f[7]; R[i][4] = -f[6];
+        const dd* e = M[4 + 2 * i] + 10;
+        const dd* f = M[5 + 2 * i] + 10;
+        const dd z = {0.0, 0.0};
+        Pd[i][0] = e[2]; Pd[i][1] = dd_sub(e[1], f[2]); Pd[i][2] = dd_sub(e[0], f[1]); Pd[i][3] = dd_sub(z, f[0]);
+        Qd[i][0] = e[5]; Qd[i][1] = dd_sub(e[4], f[5]); Qd[i][2] = dd_sub(e[3], f[4]); Qd[i][3] = dd_sub(z, f[3]);
+        Rd[i][0] = e[9]; Rd[i][1] = dd_sub(e[8], f[9]); Rd[i][2] = dd_sub(e[7], f[8]); Rd[i][3] = dd_sub(e[6], f[7]); Rd[i][4] = dd_sub(z, f[6]);
+        for (int c = 0; c < 4; c++) { P[i][c] = Pd[i][c].hi; Qp[i][c] = Qd[i][c].hi; }
+        for (int c = 0; c < 5; c++) R[i][c] = Rd[i][c].hi;
     }
-    double t1[8], t2[8], m0[8], m1[8], m2[7], d0[11], d1[11], d2[11], poly[11];
-    pmul(Qp[1], 4, R[2], 5, t1); pmul(Qp[2], 4, R[1], 5, t2);
-    for (int k = 0; k < 8; k++) m0[k] = t1[k] - t2[k];
-    pmul(P[1], 4, R[2], 5, t1); pmul(P[2], 4, R[1], 5, t2);
-    for (int k = 0; k < 8; k++) m1[k] = t1[k] - t2[k];
-    pmul(P[1], 4, Qp[2], 4, t1); pmul(P[2], 4, Qp[1], 4, t2);
-    for (int k = 0; k < 7; k++) m2[k] = t1[k] - t2[k];
-    pmul(P[0], 4, m0, 8, d0); pmul(Qp[0], 4, m1, 8, d1); pmul(R[0], 5, m2, 7, d2);
-    for (int k = 0; k < 11; k++) poly[k] = (d0[k] - d1[k]) + d2[k];
+    dd m0[8], m1[8], m2[7];
+    for (int k = 0; k < 8; k++) {
+        m0[k] = dd_sub(dd_conv(Qd[1], 4, Rd[2], 5, k), dd_conv(Qd[2], 4, Rd[1], 5, k));
+        m1[k] = dd_sub(dd_conv(Pd[1], 4, Rd[2], 5, k), dd_conv(Pd[2], 4, Rd[1], 5, k));
+        if (k < 7) m2[k] = dd_sub(dd_conv(Pd[1], 4, Qd[2], 4, k), dd_conv(Pd[2], 4, Qd[1], 4, k));
+    }
+    dd poly[11];
+    for (int k = 0; k < 11; k++)
+        poly[k] = dd_add(dd_sub(dd_conv(Pd[0], 4, m0, 8, k), dd_conv(Qd[0], 4, m1, 8, k)), dd_conv(Rd[0], 5, m2, 7, k));
     /* e. */
     double roots[10];
     const int nr = real_roots(poly, roots);

@@ -61,6 +61,29 @@ def test_essential_kernel_on_host_emulator(emu_exe, params):
     assert out.stdout.count("  ok") == 2 * len(jobs) and "FAIL" not in out.stdout and "all ok" in out.stdout, out.stdout
 
 
+def test_essential_kernel_on_named_regressions(emu_exe):
+    """parity on the five-point sets of essential_common.REGRESSIONS at m == 5, where the call returns every solution: the kernel body
+    bit for bit against the oracle. Points are float32, so the noise-free sets are their float32-rounded neighbours (identity
+    intrinsics), not the exact doubles of tests/test_essential_ref.py; with the determinant in double it lost a pair on two of them
+    and left solutions up to 7e-7 off on two others. tests/test_gpu_essential_ref.py checks these sets against the reference."""
+    exe, tmp = emu_exe
+    jobs = []
+    for name, (family, seed, k, _) in ec.REGRESSIONS.items():
+        if family == "generator":
+            rng = np.random.default_rng(seed)
+            for j in range(k + 1):
+                p1, p2 = ec.scene(rng, 5, 0.0, 0.5, "side" if j % 2 else "forward", rot=0.1)
+            jobs.append((p1, p2, None, (ec.FX, ec.FY, ec.CX, ec.CY)))
+            continue
+        q, _ = ec.regression_set(name, as_float32=True)
+        jobs.append((q[:, :2].astype(np.float32), q[:, 2:].astype(np.float32), None, (1.0, 1.0, 0.0, 0.0)))
+    path = str(tmp / "jobs_regressions.bin")
+    _write_jobs(path, jobs, 0.999, 1.0, 1000)
+    out = subprocess.run([exe, path], capture_output=True, text=True, timeout=1800)
+    assert out.returncode == 0, out.stdout + out.stderr
+    assert out.stdout.count("  ok") == 2 * len(jobs) and "FAIL" not in out.stdout and "all ok" in out.stdout, out.stdout
+
+
 def test_ctypes_essential_job_matches_the_header(tmp_path):
     sys.path.insert(0, ROOT)
     from hybvio_b200 import capi
