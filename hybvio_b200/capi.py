@@ -115,6 +115,14 @@ ESSENTIAL_MAX_POINTS = 4096    # HV_ESSENTIAL_MAX_POINTS
 ESSENTIAL_MAX_ITERS = 4096     # HV_ESSENTIAL_MAX_ITERS
 
 
+class PoseJob(ctypes.Structure):
+    """hv_pose_job: one session's essential matrix, correspondences, intrinsics and outputs in the batched relative pose (see
+    pose_job)"""
+    _fields_ = [("d_E", c_void_p), ("d_nsol", c_void_p), ("d_xy1", c_void_p), ("d_xy2", c_void_p), ("d_mask_in", c_void_p), ("n", c_int),
+                ("fx", c_double), ("fy", c_double), ("cx", c_double), ("cy", c_double),
+                ("d_R", c_void_p), ("d_t", c_void_p), ("d_mask_out", c_void_p), ("d_good", c_void_p)]
+
+
 class IngestJob(ctypes.Structure):
     """hv_ingest_job: one frame of hv_ingest_frames (see ingest_job)"""
     _fields_ = [("ing", c_void_p), ("src", c_void_p), ("stride_bytes", c_size_t), ("channels", c_int), ("coeff", c_void_p),
@@ -181,6 +189,11 @@ def load():
                                       c_double, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
     lib.hv_find_essential_device.argtypes = lib.hv_find_essential.argtypes
     lib.hv_find_essential_batch_device.argtypes = [c_void_p, ctypes.POINTER(EssentialJob), c_int, c_double, c_double, c_int]
+    lib.hv_recover_pose.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_double, c_double, c_double, c_double,
+                                    c_double, c_void_p, c_void_p, c_void_p, c_void_p]
+    lib.hv_recover_pose_device.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_double, c_double,
+                                           c_double, c_double, c_double, c_void_p, c_void_p, c_void_p, c_void_p]
+    lib.hv_recover_pose_batch_device.argtypes = [c_void_p, ctypes.POINTER(PoseJob), c_int, c_double]
     _bind_ekf(lib)
     _lib = lib
     return lib
@@ -440,6 +453,43 @@ class Context:
         J = (EssentialJob * len(jobs))(*jobs)
         check(self.lib.hv_find_essential_batch_device(self.h, J, len(jobs), prob, threshold, max_iters), "hv_find_essential_batch_device")
 
+    # ---- cv::recoverPose(E, xy1, xy2, K, R, t, distance_thresh, mask): one launch per call
+    def recover_pose(self, E, xy1, xy2, fx, fy, cx, cy, distance_thresh=50.0, mask=None):
+        """hv_recover_pose on host arrays: E (3, 3) row-major, xy1, xy2 (n, 2) float32 (converted), mask (n,) or (n, 1) uint8 or None.
+        Returns (good, R (3, 3), t (3, 1), mask (n, 1) uint8) as cv2.recoverPose returns them: the mask holds mask's value where a
+        point is good (255 without a mask), 0 elsewhere."""
+        E = np.asarray(E, np.float64)
+        if E.shape != (3, 3):
+            raise ValueError(f"E {E.shape} is not (3, 3) (cv2.recoverPose refuses a stacked E; pass its first matrix)")
+        Ecm = np.ascontiguousarray(E.T)
+        a = np.ascontiguousarray(xy1, np.float32).reshape(-1, 2)
+        b = np.ascontiguousarray(xy2, np.float32).reshape(-1, 2)
+        if a.shape != b.shape:
+            raise ValueError(f"xy1 {a.shape} and xy2 {b.shape} differ")
+        n = a.shape[0]
+        mi = None if mask is None else np.ascontiguousarray(mask, np.uint8).reshape(-1)
+        if mi is not None and mi.shape != (n,):
+            raise ValueError(f"mask {np.shape(mask)} does not hold {n} points")
+        R, t = np.zeros(9, np.float64), np.zeros(3, np.float64)
+        out = np.zeros(max(n, 1), np.uint8)
+        good = ctypes.c_int()
+        check(self.lib.hv_recover_pose(self.h, _ptr(Ecm), _ptr(a), _ptr(b), _ptr(mi), n, fx, fy, cx, cy, distance_thresh, _ptr(R), _ptr(t),
+                                       _ptr(out), ctypes.byref(good)), "hv_recover_pose")
+        keep = np.uint8(255) if mi is None else mi
+        return good.value, R.reshape(3, 3).T.copy(), t.reshape(3, 1), np.where(out[:n] != 0, keep, 0).astype(np.uint8).reshape(n, 1)
+
+    def recover_pose_device(self, d_E, d_xy1, d_xy2, d_R, d_t, d_mask_out, d_good, fx, fy, cx, cy, distance_thresh=50.0, d_nsol=None,
+                            d_mask_in=None, n=None):
+        """hv_recover_pose_device on CUDA tensors (see pose_job for the buffers); asynchronous on the context's stream."""
+        j = pose_job(d_E, d_xy1, d_xy2, d_R, d_t, d_mask_out, d_good, fx, fy, cx, cy, d_nsol, d_mask_in, n)
+        check(self.lib.hv_recover_pose_device(self.h, j.d_E, j.d_nsol, j.d_xy1, j.d_xy2, j.d_mask_in, j.n, fx, fy, cx, cy, distance_thresh,
+                                              j.d_R, j.d_t, j.d_mask_out, j.d_good), "hv_recover_pose_device")
+
+    def recover_pose_batch_device(self, jobs, distance_thresh=50.0):
+        """hv_recover_pose_batch_device: every job (see pose_job) in one launch; asynchronous."""
+        J = (PoseJob * len(jobs))(*jobs)
+        check(self.lib.hv_recover_pose_batch_device(self.h, J, len(jobs), distance_thresh), "hv_recover_pose_batch_device")
+
     def lk_track_device(self, prev, nxt, d_prev, d_next, d_status, d_ts, n, use_initial, max_iter=20, eps=0.03, min_eig=1e-3):
         check(self.lib.hv_lk_track_device(self.h, prev.h, nxt.h, _ptr(d_prev), _ptr(d_next), _ptr(d_status), _ptr(d_ts), n,
                                           1 if use_initial else 0, max_iter, eps, min_eig), "hv_lk_track_device")
@@ -518,6 +568,24 @@ def essential_job(d_xy1, d_xy2, d_E, d_nsol, d_mask, d_inliers, fx, fy, cx, cy, 
     if d_xy2.numel() // 2 < n or d_mask.numel() < n or d_E.numel() < 90 or (d_status is not None and d_status.numel() < n) or n > cap:
         raise ValueError("essential_job: a buffer is smaller than n points (or E smaller than 90 doubles)")
     return EssentialJob(_ptr(d_xy1), _ptr(d_xy2), _ptr(d_status), n, fx, fy, cx, cy, _ptr(d_E), _ptr(d_nsol), _ptr(d_mask), _ptr(d_inliers))
+
+
+def pose_job(d_E, d_xy1, d_xy2, d_R, d_t, d_mask_out, d_good, fx, fy, cx, cy, d_nsol=None, d_mask_in=None, n=None):
+    """A PoseJob on contiguous CUDA tensors: d_E float64 (at least 9: column-major, the first slot is used), d_nsol (1,) int32 or None
+    (E holds one matrix), d_xy1, d_xy2 (capacity, 2) float32, d_mask_in (capacity,) uint8 or None, d_R (9,) or (3, 3) float64
+    (column-major), d_t (3,) float64, d_mask_out (capacity,) uint8 (may be d_mask_in), d_good (1,) int32; n: the first n points (all).
+    The tensors must outlive the call that uses the job."""
+    opt = tuple((t, s) for t, s in ((d_nsol, 4), (d_mask_in, 1)) if t is not None)
+    for t, size in ((d_E, 8), (d_xy1, 4), (d_xy2, 4), (d_R, 8), (d_t, 8), (d_mask_out, 1), (d_good, 4)) + opt:
+        if not t.is_cuda or not t.is_contiguous() or t.element_size() != size:
+            raise ValueError("pose_job: every buffer must be a contiguous CUDA tensor of the documented dtype")
+    cap = d_xy1.numel() // 2
+    n = cap if n is None else n
+    if (d_xy2.numel() // 2 < n or d_mask_out.numel() < n or (d_mask_in is not None and d_mask_in.numel() < n) or n > cap
+            or d_E.numel() < 9 or d_R.numel() < 9 or d_t.numel() < 3):
+        raise ValueError("pose_job: a buffer is smaller than n points (or E, R, t smaller than 9, 9, 3 doubles)")
+    return PoseJob(_ptr(d_E), _ptr(d_nsol), _ptr(d_xy1), _ptr(d_xy2), _ptr(d_mask_in), n, fx, fy, cx, cy, _ptr(d_R), _ptr(d_t),
+                   _ptr(d_mask_out), _ptr(d_good))
 
 
 def _dense_rows(img):

@@ -1171,6 +1171,106 @@ int hv_find_essential_batch_device(hv_ctx* c, const hv_essential_job* jobs, int 
     return HV_OK;
 }
 
+// ------------------------------------------------------------------------------------------------ relative pose from E (N3)
+// Checks one job and fills its arguments; the intrinsics are refused as ess_args refuses them.
+static int pose_args(const char* who, const double* E, const int* nsol, const float* xy1, const float* xy2, const uint8_t* maskIn, int n,
+                     double fx, double fy, double cx, double cy, double* R, double* t, uint8_t* maskOut, int* good, PoseArgs& a)
+{
+    if (!E || !R || !t || !good) { hv_set_error("%s: NULL E, R, t or good", who); return HV_ERR_INVALID; }
+    if (n < 0) { hv_set_error("%s: n = %d", who, n); return HV_ERR_INVALID; }
+    if (n > 0 && (!xy1 || !xy2 || !maskOut)) { hv_set_error("%s: NULL xy1, xy2 or mask_out", who); return HV_ERR_INVALID; }
+    if (n > HV_ESSENTIAL_MAX_POINTS) { hv_set_error("%s: %d points (at most %d)", who, n, HV_ESSENTIAL_MAX_POINTS); return HV_ERR_UNSUPPORTED; }
+    if (!std::isfinite(fx) || !std::isfinite(fy) || !std::isfinite(cx) || !std::isfinite(cy) || fx == 0.0 || fy == 0.0) {
+        hv_set_error("%s: intrinsics (%g, %g, %g, %g) not finite or a zero focal length", who, fx, fy, cx, cy);
+        return HV_ERR_UNSUPPORTED;
+    }
+    memset(&a, 0, sizeof(a));
+    a.E = E; a.nsol = nsol;
+    a.xy1 = (const float2*)xy1; a.xy2 = (const float2*)xy2; a.maskIn = maskIn; a.n = n;
+    a.fx = fx; a.fy = fy; a.cx = cx; a.cy = cy;
+    a.R = R; a.t = t; a.maskOut = maskOut; a.good = good;
+    return HV_OK;
+}
+
+int hv_recover_pose_device(hv_ctx* c, const double* dE, const int* dNsol, const float* dXY1, const float* dXY2, const uint8_t* dMaskIn, int n,
+                           double fx, double fy, double cx, double cy, double dist, double* dR, double* dT, uint8_t* dMaskOut, int* dGood)
+{
+    const char* who = "hv_recover_pose_device";
+    if (!c) { hv_set_error("%s: NULL context", who); return HV_ERR_INVALID; }
+    PoseBatchArgs b;
+    memset(&b, 0, sizeof(b));
+    int rc = pose_args(who, dE, dNsol, dXY1, dXY2, dMaskIn, n, fx, fy, cx, cy, dR, dT, dMaskOut, dGood, b.job[0]);
+    if (rc != HV_OK) return rc;
+    b.dist = dist;
+    HV_CUDA(cudaSetDevice(c->device));
+    HV_CUDA(hv_launch_pose(b, 1, c->stream));
+    c->launches += 1;
+    return HV_OK;
+}
+
+int hv_recover_pose(hv_ctx* c, const double* E, const float* xy1, const float* xy2, const uint8_t* maskIn, int n, double fx, double fy,
+                    double cx, double cy, double dist, double* R, double* t, uint8_t* maskOut, int* good)
+{
+    const char* who = "hv_recover_pose";
+    if (!c) { hv_set_error("%s: NULL context", who); return HV_ERR_INVALID; }
+    PoseBatchArgs b;
+    memset(&b, 0, sizeof(b));
+    int rc = pose_args(who, E, nullptr, xy1, xy2, maskIn, n, fx, fy, cx, cy, R, t, maskOut, good, b.job[0]);
+    if (rc != HV_OK) return rc;
+    for (int k = 0; k < 9; k++)
+        if (!std::isfinite(E[k])) { hv_set_error("%s: E[%d] = %g is not finite", who, k, E[k]); return HV_ERR_UNSUPPORTED; }
+    b.dist = dist;
+    HV_CUDA(cudaSetDevice(c->device));
+    // staging block: [R 9 | t 3 doubles | good | mask_out n] back to the host, [E 9 doubles | xy1 8n | xy2 8n | mask_in n] to the device
+    const size_t oGood = 8 * 12, oMask = oGood + 16, oE = align_up(oMask + (size_t)n, 16), oXY1 = oE + 8 * 9;
+    const size_t oXY2 = oXY1 + 8 * (size_t)n, oMi = oXY2 + 8 * (size_t)n, total = oMi + (maskIn ? (size_t)n : 0);
+    rc = hv_ctx_reserve_stage(c, total);
+    if (rc != HV_OK) return rc;
+    uint8_t* hs = (uint8_t*)c->h_stage; uint8_t* ds = (uint8_t*)c->d_stage;
+    memcpy(hs + oE, E, 8 * 9);
+    if (n > 0) {
+        memcpy(hs + oXY1, xy1, 8 * (size_t)n);
+        memcpy(hs + oXY2, xy2, 8 * (size_t)n);
+        if (maskIn) memcpy(hs + oMi, maskIn, (size_t)n);
+    }
+    HV_CUDA(cudaMemcpyAsync(ds + oE, hs + oE, total - oE, cudaMemcpyHostToDevice, c->stream));
+    PoseArgs& a = b.job[0];
+    a.E = (const double*)(ds + oE); a.xy1 = (const float2*)(ds + oXY1); a.xy2 = (const float2*)(ds + oXY2);
+    a.maskIn = maskIn ? ds + oMi : nullptr;
+    a.R = (double*)ds; a.t = (double*)(ds + 8 * 9); a.good = (int*)(ds + oGood); a.maskOut = ds + oMask;
+    HV_CUDA(hv_launch_pose(b, 1, c->stream));
+    c->launches += 1;
+    HV_CUDA(cudaMemcpyAsync(hs, ds, oMask + (size_t)n, cudaMemcpyDeviceToHost, c->stream));
+    HV_CUDA(cudaStreamSynchronize(c->stream));
+    memcpy(R, hs, 8 * 9);
+    memcpy(t, hs + 8 * 9, 8 * 3);
+    memcpy(good, hs + oGood, sizeof(int));
+    if (n > 0) memcpy(maskOut, hs + oMask, (size_t)n);
+    return HV_OK;
+}
+
+int hv_recover_pose_batch_device(hv_ctx* c, const hv_pose_job* jobs, int njobs, double dist)
+{
+    const char* who = "hv_recover_pose_batch_device";
+    if (!c || !jobs) { hv_set_error("%s: NULL context or jobs", who); return HV_ERR_INVALID; }
+    if (njobs < 1 || njobs > HV_ESSENTIAL_BATCH_MAX) { hv_set_error("%s: %d jobs (1..%d per call)", who, njobs, HV_ESSENTIAL_BATCH_MAX); return HV_ERR_INVALID; }
+    PoseBatchArgs b;
+    memset(&b, 0, sizeof(b));
+    for (int j = 0; j < njobs; j++) {
+        const hv_pose_job& J = jobs[j];
+        char w[64];
+        snprintf(w, sizeof(w), "%s job %d", who, j);
+        const int rc = pose_args(w, J.d_E, J.d_nsol, J.d_xy1, J.d_xy2, J.d_mask_in, J.n, J.fx, J.fy, J.cx, J.cy, J.d_R, J.d_t, J.d_mask_out,
+                                 J.d_good, b.job[j]);
+        if (rc != HV_OK) return rc;
+    }
+    b.dist = dist;
+    HV_CUDA(cudaSetDevice(c->device));
+    HV_CUDA(hv_launch_pose(b, njobs, c->stream));
+    c->launches += 1;
+    return HV_OK;
+}
+
 // ------------------------------------------------------------------------------------------------ frame ingest (N4)
 struct hv_ingest {
     hv_ctx* ctx = nullptr;

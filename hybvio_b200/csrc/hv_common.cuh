@@ -244,6 +244,24 @@ struct EssentialBatchArgs {
 static_assert(sizeof(EssentialBatchArgs) <= HV_KERNEL_PARAM_MAX, "essential batch arguments exceed the kernel-parameter space");
 cudaError_t hv_launch_essential(const EssentialBatchArgs& b, int njobs, cudaStream_t stream);     // one launch, one CTA per job
 
+// ---- relative pose (pose.cu): cv::recoverPose(E, xy1, xy2, K, R, t, distanceThresh, mask), up to HV_ESSENTIAL_BATCH_MAX jobs
+struct PoseArgs {
+    const double* E;                  // column-major 3 x 3 slots; the first is used
+    const int* nsol;                  // NULL: E is one matrix; *nsol == 0: no result (R, t, mask and good zero)
+    const float2* xy1; const float2* xy2;
+    const uint8_t* maskIn;            // NULL: every point is used
+    int n;
+    double fx, fy, cx, cy;
+    double* R; double* t;             // column-major 3 x 3, 3
+    uint8_t* maskOut; int* good;      // maskOut 0/1, may be maskIn
+};
+struct PoseBatchArgs {
+    PoseArgs job[HV_ESSENTIAL_BATCH_MAX];
+    double dist;
+};
+static_assert(sizeof(PoseBatchArgs) <= HV_KERNEL_PARAM_MAX, "pose batch arguments exceed the kernel-parameter space");
+cudaError_t hv_launch_pose(const PoseBatchArgs& b, int njobs, cudaStream_t stream);     // one launch, one CTA per job
+
 // ---- frame ingest (ingest.cu)
 #define HV_REMAP_INVALID (-32768)
 struct HvRemapEntry { short x0, y0; float xfrac, yfrac; };      // 12 bytes per output pixel (hv_remap_entry of the C ABI)

@@ -312,6 +312,41 @@ typedef struct hv_essential_job {
 } hv_essential_job;
 int hv_find_essential_batch_device(hv_ctx* ctx, const hv_essential_job* jobs, int njobs, double prob, double threshold, int max_iters);
 
+/* ---------------------------------------------------------------- relative pose from E (SURVEY.md 8(f) N3) -- */
+/* cv::recoverPose(E, xy1, xy2, K, R, t, distance_thresh, mask) (OCV/calib3d/src/five-point.cpp): decomposeEssentialMat's four
+ * candidates [R1 | t], [R2 | t], [R1 | -t], [R2 | -t]; every point triangulated (DLT) under each; a point is good for a candidate when
+ * its depth in both cameras is positive and below distance_thresh, and mask_in (if any) is non-zero there; the candidate with the most
+ * good points wins, ties going to the first in that order, as in OpenCV. K = [[fx, 0, cx], [0, fy, cy], [0, 0, 1]]. Both SVDs are this
+ * library's own (DESIGN.md 4.12), so where two candidates tie at the winning count, OpenCV's choice between them (its SVD's sign
+ * conventions) can be the other one; wherever one candidate wins alone the result is OpenCV's.
+ *   E         column-major fp64 3 x 3 (host call: one matrix). d_nsol (device calls) NULL: d_E is one matrix; otherwise the count
+ *             hv_find_essential_device wrote: 0 gives good 0, a zero mask and R = t = 0; above 1 the first slot is used, which is
+ *             cv::recoverPose(E[0:3]) (OpenCV refuses the stacked matrix)
+ *   xy1, xy2  n x (x, y) float32, as hv_find_essential takes them; every point is triangulated
+ *   mask_in   n x u8 or NULL (every point used); mask_out n x u8: 1 where the point is good for the winner (0 where mask_in is 0);
+ *             mask_out may be mask_in, so hv_find_essential_device's d_mask can be refined in place
+ *   R, t      the winner, column-major fp64 3 x 3 and 3; good its count
+ * distance_thresh may be any value OpenCV accepts (50 is its default); NaN passes no point.
+ * Errors, before anything is launched (buffers and the context's launch count untouched): HV_ERR_INVALID for a NULL context / E / R /
+ * t / good, a NULL xy1 / xy2 / mask_out with n > 0, n < 0; HV_ERR_UNSUPPORTED for n above HV_ESSENTIAL_MAX_POINTS and intrinsics that
+ * are not finite or have a zero focal length, and (host call) an E that is not finite. Every call is one launch. */
+int hv_recover_pose(hv_ctx* ctx, const double* E, const float* xy1, const float* xy2, const uint8_t* mask_in, int n, double fx, double fy,
+                    double cx, double cy, double distance_thresh, double* R, double* t, uint8_t* mask_out, int* good); /* host, synchronises */
+int hv_recover_pose_device(hv_ctx* ctx, const double* d_E, const int* d_nsol, const float* d_xy1, const float* d_xy2,
+                           const uint8_t* d_mask_in, int n, double fx, double fy, double cx, double cy, double distance_thresh, double* d_R,
+                           double* d_t, uint8_t* d_mask_out, int* d_good);                                   /* device, asynchronous */
+/* hv_recover_pose_device for 1..HV_ESSENTIAL_BATCH_MAX jobs in the one launch of one call: every job's outputs are bit-identical to the
+ * per-call function's. Everything but distance_thresh is per job. Errors as hv_recover_pose_device's for every job, and HV_ERR_INVALID
+ * for a NULL jobs array or njobs outside 1..HV_ESSENTIAL_BATCH_MAX, all before anything is launched. */
+typedef struct hv_pose_job {
+    const double* d_E; const int* d_nsol;
+    const float* d_xy1; const float* d_xy2; const uint8_t* d_mask_in;
+    int n;
+    double fx, fy, cx, cy;
+    double* d_R; double* d_t; uint8_t* d_mask_out; int* d_good;
+} hv_pose_job;
+int hv_recover_pose_batch_device(hv_ctx* ctx, const hv_pose_job* jobs, int njobs, double distance_thresh);
+
 /* ---------------------------------------------------------------- frame ingest (SURVEY.md 8(f) N4) -------- */
 /* Device part of tracker::Image::Factory::build / buildStereo (src/tracker/image.cpp:243-308): colour -> gray
  * (accelerated-arrays pixelwiseAffine, image.cpp:360-366) and undistortion / rectification (UndistorterImplementation::undistort,
