@@ -115,6 +115,16 @@ ESSENTIAL_MAX_POINTS = 4096    # HV_ESSENTIAL_MAX_POINTS
 ESSENTIAL_MAX_ITERS = 4096     # HV_ESSENTIAL_MAX_ITERS
 
 
+class PnpJob(ctypes.Structure):
+    """hv_pnp_job: one session's 3-D points, pixels, intrinsics and outputs in the batched absolute-pose RANSAC (see pnp_job)"""
+    _fields_ = [("d_xyz", c_void_p), ("d_xy", c_void_p), ("d_status", c_void_p), ("n", c_int),
+                ("fx", c_double), ("fy", c_double), ("cx", c_double), ("cy", c_double),
+                ("d_rvec", c_void_p), ("d_tvec", c_void_p), ("d_mask", c_void_p), ("d_inliers", c_void_p), ("d_ok", c_void_p)]
+
+
+PNP_MAX_POINTS = 4096          # HV_PNP_MAX_POINTS
+PNP_MAX_ITERS = 4096           # HV_PNP_MAX_ITERS
+
 class PoseJob(ctypes.Structure):
     """hv_pose_job: one session's essential matrix, correspondences, intrinsics and outputs in the batched relative pose (see
     pose_job)"""
@@ -194,6 +204,10 @@ def load():
     lib.hv_recover_pose_device.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_double, c_double,
                                            c_double, c_double, c_double, c_void_p, c_void_p, c_void_p, c_void_p]
     lib.hv_recover_pose_batch_device.argtypes = [c_void_p, ctypes.POINTER(PoseJob), c_int, c_double]
+    lib.hv_solve_pnp_ransac.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_double, c_double, c_double, c_double, c_int,
+                                        ctypes.c_float, c_double, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
+    lib.hv_solve_pnp_ransac_device.argtypes = lib.hv_solve_pnp_ransac.argtypes
+    lib.hv_solve_pnp_ransac_batch_device.argtypes = [c_void_p, ctypes.POINTER(PnpJob), c_int, c_int, ctypes.c_float, c_double]
     _bind_ekf(lib)
     _lib = lib
     return lib
@@ -453,6 +467,40 @@ class Context:
         J = (EssentialJob * len(jobs))(*jobs)
         check(self.lib.hv_find_essential_batch_device(self.h, J, len(jobs), prob, threshold, max_iters), "hv_find_essential_batch_device")
 
+    # ---- cv::solvePnPRansac(..., SOLVEPNP_P3P): one launch per call
+    def solve_pnp_ransac(self, xyz, xy, fx, fy, cx, cy, iterations=100, reproj_error=8.0, confidence=0.99, status=None):
+        """hv_solve_pnp_ransac on host arrays: xyz (n, 3) and xy (n, 2) float32 (converted), status (n,) uint8 or None. Returns
+        (ok, rvec, tvec, inliers) as cv2.solvePnPRansac(..., flags=cv2.SOLVEPNP_P3P) returns them: ok bool, rvec and tvec (3, 1) float64,
+        inliers (k, 1) int32 indices into the n points, or None when there are none."""
+        X = np.ascontiguousarray(xyz, np.float32).reshape(-1, 3)
+        x = np.ascontiguousarray(xy, np.float32).reshape(-1, 2)
+        if X.shape[0] != x.shape[0]:
+            raise ValueError(f"xyz {X.shape} and xy {x.shape} hold different point counts")
+        n = X.shape[0]
+        st = None if status is None else np.ascontiguousarray(status, np.uint8)
+        if st is not None and st.shape != (n,):
+            raise ValueError(f"status {st.shape} is not ({n},)")
+        r, t = np.zeros(3), np.zeros(3)
+        mask = np.zeros(max(n, 1), np.uint8)
+        inl, ok = ctypes.c_int(), ctypes.c_int()
+        check(self.lib.hv_solve_pnp_ransac(self.h, _ptr(X), _ptr(x), _ptr(st), n, fx, fy, cx, cy, iterations, reproj_error, confidence,
+                                           _ptr(r), _ptr(t), _ptr(mask), ctypes.byref(inl), ctypes.byref(ok)), "hv_solve_pnp_ransac")
+        idx = np.flatnonzero(mask[:n]).astype(np.int32).reshape(-1, 1)
+        return bool(ok.value), r.reshape(3, 1), t.reshape(3, 1), (idx if ok.value and idx.size else None)
+
+    def solve_pnp_ransac_device(self, d_xyz, d_xy, d_rvec, d_tvec, d_mask, d_inliers, d_ok, fx, fy, cx, cy, iterations=100,
+                                reproj_error=8.0, confidence=0.99, d_status=None, n=None):
+        """hv_solve_pnp_ransac_device on CUDA tensors (see pnp_job for the buffers); asynchronous on the context's stream."""
+        j = pnp_job(d_xyz, d_xy, d_rvec, d_tvec, d_mask, d_inliers, d_ok, fx, fy, cx, cy, d_status, n)
+        check(self.lib.hv_solve_pnp_ransac_device(self.h, j.d_xyz, j.d_xy, j.d_status, j.n, fx, fy, cx, cy, iterations, reproj_error,
+                                                  confidence, j.d_rvec, j.d_tvec, j.d_mask, j.d_inliers, j.d_ok), "hv_solve_pnp_ransac_device")
+
+    def solve_pnp_ransac_batch_device(self, jobs, iterations=100, reproj_error=8.0, confidence=0.99):
+        """hv_solve_pnp_ransac_batch_device: every job (see pnp_job) in one launch; asynchronous."""
+        J = (PnpJob * len(jobs))(*jobs)
+        check(self.lib.hv_solve_pnp_ransac_batch_device(self.h, J, len(jobs), iterations, reproj_error, confidence),
+              "hv_solve_pnp_ransac_batch_device")
+
     # ---- cv::recoverPose(E, xy1, xy2, K, R, t, distance_thresh, mask): one launch per call
     def recover_pose(self, E, xy1, xy2, fx, fy, cx, cy, distance_thresh=50.0, mask=None):
         """hv_recover_pose on host arrays: E (3, 3) row-major, xy1, xy2 (n, 2) float32 (converted), mask (n,) or (n, 1) uint8 or None.
@@ -569,6 +617,21 @@ def essential_job(d_xy1, d_xy2, d_E, d_nsol, d_mask, d_inliers, fx, fy, cx, cy, 
         raise ValueError("essential_job: a buffer is smaller than n points (or E smaller than 90 doubles)")
     return EssentialJob(_ptr(d_xy1), _ptr(d_xy2), _ptr(d_status), n, fx, fy, cx, cy, _ptr(d_E), _ptr(d_nsol), _ptr(d_mask), _ptr(d_inliers))
 
+
+def pnp_job(d_xyz, d_xy, d_rvec, d_tvec, d_mask, d_inliers, d_ok, fx, fy, cx, cy, d_status=None, n=None):
+    """A PnpJob on contiguous CUDA tensors: d_xyz (capacity, 3) float32, d_xy (capacity, 2) float32, d_status (capacity,) uint8 or None,
+    d_rvec and d_tvec (3,) float64, d_mask (capacity,) uint8, d_inliers and d_ok (1,) int32; n: the first n points (all).
+    The tensors must outlive the call that uses the job."""
+    for t, size in ((d_xyz, 4), (d_xy, 4), (d_rvec, 8), (d_tvec, 8), (d_mask, 1), (d_inliers, 4), (d_ok, 4)) + (() if d_status is None else ((d_status, 1),)):
+        if not t.is_cuda or not t.is_contiguous() or t.element_size() != size:
+            raise ValueError("pnp_job: every buffer must be a contiguous CUDA tensor of the documented dtype")
+    cap = d_xyz.numel() // 3
+    n = cap if n is None else n
+    if (d_xy.numel() // 2 < n or d_mask.numel() < n or (d_status is not None and d_status.numel() < n) or n > cap
+            or d_rvec.numel() < 3 or d_tvec.numel() < 3):
+        raise ValueError("pnp_job: a buffer is smaller than n points (or rvec, tvec smaller than 3 doubles)")
+    return PnpJob(_ptr(d_xyz), _ptr(d_xy), _ptr(d_status), n, fx, fy, cx, cy, _ptr(d_rvec), _ptr(d_tvec), _ptr(d_mask), _ptr(d_inliers),
+                  _ptr(d_ok))
 
 def pose_job(d_E, d_xy1, d_xy2, d_R, d_t, d_mask_out, d_good, fx, fy, cx, cy, d_nsol=None, d_mask_in=None, n=None):
     """A PoseJob on contiguous CUDA tensors: d_E float64 (at least 9: column-major, the first slot is used), d_nsol (1,) int32 or None

@@ -1064,11 +1064,9 @@ static int ess_args(const char* who, const float* xy1, const float* xy2, const u
     return HV_OK;
 }
 
-// points the jobs' normalised points and indices into the context's scratch, grown (after the work that may still read it) as needed
-static int ess_scratch(hv_ctx* c, EssentialArgs* jobs, int njobs)
+// grows the context's scratch (hv_find_essential*, hv_solve_pnp_ransac*) to `total` bytes, after the work that may still read it
+static int ctx_scratch(hv_ctx* c, size_t total)
 {
-    size_t total = 0;
-    for (int j = 0; j < njobs; j++) total += align_up(32 * (size_t)jobs[j].n, 256) + align_up(4 * (size_t)jobs[j].n, 256);
     if (total > c->essScratchBytes) {
         if (c->d_essScratch) { HV_CUDA(cudaStreamSynchronize(c->stream)); cudaFree(c->d_essScratch); }
         c->d_essScratch = nullptr; c->essScratchBytes = 0;
@@ -1076,6 +1074,16 @@ static int ess_scratch(hv_ctx* c, EssentialArgs* jobs, int njobs)
         HV_CUDA(cudaMalloc(&c->d_essScratch, cap));
         c->essScratchBytes = cap;
     }
+    return HV_OK;
+}
+
+// points the jobs' normalised points and indices into the context's scratch, grown as needed
+static int ess_scratch(hv_ctx* c, EssentialArgs* jobs, int njobs)
+{
+    size_t total = 0;
+    for (int j = 0; j < njobs; j++) total += align_up(32 * (size_t)jobs[j].n, 256) + align_up(4 * (size_t)jobs[j].n, 256);
+    const int rc = ctx_scratch(c, total);
+    if (rc != HV_OK) return rc;
     uint8_t* p = (uint8_t*)c->d_essScratch;
     for (int j = 0; j < njobs; j++) {
         jobs[j].q = (double*)p; p += align_up(32 * (size_t)jobs[j].n, 256);
@@ -1267,6 +1275,151 @@ int hv_recover_pose_batch_device(hv_ctx* c, const hv_pose_job* jobs, int njobs, 
     b.dist = dist;
     HV_CUDA(cudaSetDevice(c->device));
     HV_CUDA(hv_launch_pose(b, njobs, c->stream));
+    c->launches += 1;
+    return HV_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ absolute-pose RANSAC (N3)
+// The parameters of the batch: refused as cv::solvePnPRansac 4.13 refuses them (confidence outside (0, 1), NaN included), or as the
+// device cannot run them (more than HV_PNP_MAX_ITERS iterations; iterations <= 0 runs one, as OpenCV does).
+static int pnp_params(const char* who, int iterations, double confidence)
+{
+    if (!(confidence > 0.0 && confidence < 1.0)) { hv_set_error("%s: confidence %g outside (0, 1)", who, confidence); return HV_ERR_INVALID; }
+    if (iterations > HV_PNP_MAX_ITERS) { hv_set_error("%s: iterations %d above %d", who, iterations, HV_PNP_MAX_ITERS); return HV_ERR_UNSUPPORTED; }
+    return HV_OK;
+}
+
+// Checks one job and fills everything but the scratch; the intrinsics are refused as ess_args refuses them.
+static int pnp_args(const char* who, const float* xyz, const float* xy, const uint8_t* status, int n, double fx, double fy, double cx,
+                    double cy, double* rvec, double* tvec, uint8_t* mask, int* inliers, int* ok, PnpArgs& a)
+{
+    if (!rvec || !tvec || !inliers || !ok) { hv_set_error("%s: NULL rvec, tvec, inliers or ok", who); return HV_ERR_INVALID; }
+    if (n < 0) { hv_set_error("%s: n = %d", who, n); return HV_ERR_INVALID; }
+    if (n > 0 && (!xyz || !xy || !mask)) { hv_set_error("%s: NULL xyz, xy or mask", who); return HV_ERR_INVALID; }
+    if (n > HV_PNP_MAX_POINTS) { hv_set_error("%s: %d points (at most %d)", who, n, HV_PNP_MAX_POINTS); return HV_ERR_UNSUPPORTED; }
+    if (!std::isfinite(fx) || !std::isfinite(fy) || !std::isfinite(cx) || !std::isfinite(cy) || fx == 0.0 || fy == 0.0) {
+        hv_set_error("%s: intrinsics (%g, %g, %g, %g) not finite or a zero focal length", who, fx, fy, cx, cy);
+        return HV_ERR_UNSUPPORTED;
+    }
+    memset(&a, 0, sizeof(a));
+    a.xyz = xyz; a.xy = (const float2*)xy; a.status = status; a.n = n;
+    a.fx = fx; a.fy = fy; a.cx = cx; a.cy = cy;
+    a.rvec = rvec; a.tvec = tvec; a.mask = mask; a.inliers = inliers; a.ok = ok;
+    return HV_OK;
+}
+
+// points the jobs' compacted points into the context's scratch (120 bytes per point), grown as needed
+static int pnp_scratch(hv_ctx* c, PnpArgs* jobs, int njobs)
+{
+    size_t total = 0;
+    for (int j = 0; j < njobs; j++) {
+        const size_t n = (size_t)jobs[j].n;
+        total += align_up(12 * n, 256) + align_up(8 * n, 256) + align_up(4 * n, 256) + align_up(24 * n, 256) + align_up(16 * n, 256) +
+                 align_up(32 * n, 256) + align_up(24 * n, 256);
+    }
+    const int rc = ctx_scratch(c, total);
+    if (rc != HV_OK) return rc;
+    uint8_t* p = (uint8_t*)c->d_essScratch;
+    for (int j = 0; j < njobs; j++) {
+        const size_t n = (size_t)jobs[j].n;
+        jobs[j].P = (float*)p; p += align_up(12 * n, 256);
+        jobs[j].Q = (float2*)p; p += align_up(8 * n, 256);
+        jobs[j].idx = (int*)p; p += align_up(4 * n, 256);
+        jobs[j].pws = (double*)p; p += align_up(24 * n, 256);
+        jobs[j].us = (double*)p; p += align_up(16 * n, 256);
+        jobs[j].al = (double*)p; p += align_up(32 * n, 256);
+        jobs[j].pcs = (double*)p; p += align_up(24 * n, 256);
+    }
+    return HV_OK;
+}
+
+int hv_solve_pnp_ransac_device(hv_ctx* c, const float* dXYZ, const float* dXY, const uint8_t* dStatus, int n, double fx, double fy,
+                               double cx, double cy, int iterations, float reprojError, double confidence, double* dRvec, double* dTvec,
+                               uint8_t* dMask, int* dInliers, int* dOk)
+{
+    const char* who = "hv_solve_pnp_ransac_device";
+    if (!c) { hv_set_error("%s: NULL context", who); return HV_ERR_INVALID; }
+    int rc = pnp_params(who, iterations, confidence);
+    if (rc != HV_OK) return rc;
+    PnpBatchArgs b;
+    memset(&b, 0, sizeof(b));
+    rc = pnp_args(who, dXYZ, dXY, dStatus, n, fx, fy, cx, cy, dRvec, dTvec, dMask, dInliers, dOk, b.job[0]);
+    if (rc != HV_OK) return rc;
+    b.iterations = iterations; b.reprojError = reprojError; b.confidence = confidence;
+    HV_CUDA(cudaSetDevice(c->device));
+    rc = pnp_scratch(c, b.job, 1);
+    if (rc != HV_OK) return rc;
+    HV_CUDA(hv_launch_pnp(b, 1, c->stream));
+    c->launches += 1;
+    return HV_OK;
+}
+
+int hv_solve_pnp_ransac(hv_ctx* c, const float* xyz, const float* xy, const uint8_t* status, int n, double fx, double fy, double cx,
+                        double cy, int iterations, float reprojError, double confidence, double* rvec, double* tvec, uint8_t* mask,
+                        int* inliers, int* ok)
+{
+    const char* who = "hv_solve_pnp_ransac";
+    if (!c) { hv_set_error("%s: NULL context", who); return HV_ERR_INVALID; }
+    int rc = pnp_params(who, iterations, confidence);
+    if (rc != HV_OK) return rc;
+    PnpBatchArgs b;
+    memset(&b, 0, sizeof(b));
+    rc = pnp_args(who, xyz, xy, status, n, fx, fy, cx, cy, rvec, tvec, mask, inliers, ok, b.job[0]);
+    if (rc != HV_OK) return rc;
+    b.iterations = iterations; b.reprojError = reprojError; b.confidence = confidence;
+    HV_CUDA(cudaSetDevice(c->device));
+    rc = pnp_scratch(c, b.job, 1);
+    if (rc != HV_OK) return rc;
+    // staging block: [rvec 3 | tvec 3 doubles | inliers, ok | mask n] back to the host, [xyz 12n | xy 8n (16-byte aligned: read as
+    // float2) | status n] to the device
+    const size_t oMask = 8 * 6 + 16, oXYZ = align_up(oMask + (size_t)n, 16);
+    const size_t oXY = align_up(oXYZ + 12 * (size_t)n, 16), oSt = oXY + 8 * (size_t)n, total = oSt + (status ? (size_t)n : 0);
+    rc = hv_ctx_reserve_stage(c, total);
+    if (rc != HV_OK) return rc;
+    uint8_t* hs = (uint8_t*)c->h_stage; uint8_t* ds = (uint8_t*)c->d_stage;
+    if (n > 0) {
+        memcpy(hs + oXYZ, xyz, 12 * (size_t)n);
+        memcpy(hs + oXY, xy, 8 * (size_t)n);
+        if (status) memcpy(hs + oSt, status, (size_t)n);
+    }
+    if (total > oXYZ) HV_CUDA(cudaMemcpyAsync(ds + oXYZ, hs + oXYZ, total - oXYZ, cudaMemcpyHostToDevice, c->stream));
+    PnpArgs& a = b.job[0];
+    a.xyz = (const float*)(ds + oXYZ); a.xy = (const float2*)(ds + oXY); a.status = status ? ds + oSt : nullptr;
+    a.rvec = (double*)ds; a.tvec = (double*)(ds + 24); a.inliers = (int*)(ds + 48); a.ok = (int*)(ds + 52); a.mask = ds + oMask;
+    HV_CUDA(hv_launch_pnp(b, 1, c->stream));
+    c->launches += 1;
+    HV_CUDA(cudaMemcpyAsync(hs, ds, oMask + (size_t)n, cudaMemcpyDeviceToHost, c->stream));
+    HV_CUDA(cudaStreamSynchronize(c->stream));
+    memcpy(rvec, hs, 24);
+    memcpy(tvec, hs + 24, 24);
+    memcpy(inliers, hs + 48, sizeof(int));
+    memcpy(ok, hs + 52, sizeof(int));
+    if (n > 0) memcpy(mask, hs + oMask, (size_t)n);
+    return HV_OK;
+}
+
+int hv_solve_pnp_ransac_batch_device(hv_ctx* c, const hv_pnp_job* jobs, int njobs, int iterations, float reprojError, double confidence)
+{
+    const char* who = "hv_solve_pnp_ransac_batch_device";
+    if (!c || !jobs) { hv_set_error("%s: NULL context or jobs", who); return HV_ERR_INVALID; }
+    if (njobs < 1 || njobs > HV_ESSENTIAL_BATCH_MAX) { hv_set_error("%s: %d jobs (1..%d per call)", who, njobs, HV_ESSENTIAL_BATCH_MAX); return HV_ERR_INVALID; }
+    int rc = pnp_params(who, iterations, confidence);
+    if (rc != HV_OK) return rc;
+    PnpBatchArgs b;
+    memset(&b, 0, sizeof(b));
+    for (int j = 0; j < njobs; j++) {
+        const hv_pnp_job& J = jobs[j];
+        char w[64];
+        snprintf(w, sizeof(w), "%s job %d", who, j);
+        rc = pnp_args(w, J.d_xyz, J.d_xy, J.d_status, J.n, J.fx, J.fy, J.cx, J.cy, J.d_rvec, J.d_tvec, J.d_mask, J.d_inliers, J.d_ok,
+                      b.job[j]);
+        if (rc != HV_OK) return rc;
+    }
+    b.iterations = iterations; b.reprojError = reprojError; b.confidence = confidence;
+    HV_CUDA(cudaSetDevice(c->device));
+    rc = pnp_scratch(c, b.job, njobs);
+    if (rc != HV_OK) return rc;
+    HV_CUDA(hv_launch_pnp(b, njobs, c->stream));
     c->launches += 1;
     return HV_OK;
 }

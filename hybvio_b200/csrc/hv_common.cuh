@@ -262,6 +262,30 @@ struct PoseBatchArgs {
 static_assert(sizeof(PoseBatchArgs) <= HV_KERNEL_PARAM_MAX, "pose batch arguments exceed the kernel-parameter space");
 cudaError_t hv_launch_pose(const PoseBatchArgs& b, int njobs, cudaStream_t stream);     // one launch, one CTA per job
 
+// ---- absolute-pose RANSAC (pnp.cu): cv::solvePnPRansac(..., SOLVEPNP_P3P) on the used points, up to HV_ESSENTIAL_BATCH_MAX jobs
+#define HV_PNP_MAX_POINTS 4096
+#define HV_PNP_MAX_ITERS 4096
+struct PnpArgs {
+    const float* xyz;                 // n x 3
+    const float2* xy;
+    const uint8_t* status;            // NULL: every point is used
+    int n;
+    double fx, fy, cx, cy;
+    double* rvec; double* tvec;       // 3 each
+    uint8_t* mask; int* inliers; int* ok;
+    float* P; float2* Q; int* idx;    // scratch: the used points (world, image) and their original indices
+    double* pws; double* us;          // scratch: EPnP's inliers (world, image after OpenCV's undistort round trip)
+    double* al; double* pcs;          // scratch: their barycentric coordinates and camera points
+};
+struct PnpBatchArgs {
+    PnpArgs job[HV_ESSENTIAL_BATCH_MAX];
+    double confidence;
+    float reprojError;
+    int iterations;
+};
+static_assert(sizeof(PnpBatchArgs) <= HV_KERNEL_PARAM_MAX, "pnp batch arguments exceed the kernel-parameter space");
+cudaError_t hv_launch_pnp(const PnpBatchArgs& b, int njobs, cudaStream_t stream);     // one launch, one CTA per job
+
 // ---- frame ingest (ingest.cu)
 #define HV_REMAP_INVALID (-32768)
 struct HvRemapEntry { short x0, y0; float xfrac, yfrac; };      // 12 bytes per output pixel (hv_remap_entry of the C ABI)

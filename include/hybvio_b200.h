@@ -347,6 +347,49 @@ typedef struct hv_pose_job {
 } hv_pose_job;
 int hv_recover_pose_batch_device(hv_ctx* ctx, const hv_pose_job* jobs, int njobs, double distance_thresh);
 
+/* ---------------------------------------------------------------- absolute-pose RANSAC (SURVEY.md 8(f) N3) -- */
+/* cv::solvePnPRansac(xyz[used], xy[used], K, noArray(), rvec, tvec, false, iterations, reproj_error, confidence, inliers, SOLVEPNP_P3P)
+ * (OCV/calib3d/src/solvepnp.cpp, ptsetreg.cpp, epnp.cpp): the pose of a camera from 3-D points and their pixels, outliers rejected --
+ * the stereo path's pose of the current frame against points triangulated from the previous stereo pair. K = [[fx, 0, cx], [0, fy, cy],
+ * [0, 0, 1]], no distortion (HybVIO's camera model hands over pinhole points), no extrinsic guess. The used points are those with
+ * status != 0 (all n when status is NULL), in index order; m is their count. RANSAC replays OpenCV's with 4-point subsets: cv::RNG seeded
+ * with ~0 draws them, the model is the P3P pose of the first three that reprojects the fourth closest, a count above max(best, 3) wins,
+ * the bound shrinks through RANSACUpdateNumIters, and a point is an inlier when its float32 squared pixel distance to its projection is
+ * <= (float)(reproj_error^2). The winner's inliers go through one EPnP in double, whose pose is returned; the returned inliers are the
+ * RANSAC model's. The P3P solver, the SVDs and the trigonometry are this library's own (DESIGN.md 4.13): the same pose as OpenCV's up
+ * to rounding, the same inliers wherever no point lies within rounding of the threshold.
+ *   xyz       n x 3 float32 world points; xy n x (x, y) float32 pixels (the layout the LK calls write)
+ *   status    n x u8 or NULL; LK's status over a padded capacity (HV_CORNER_NONE slots report 0) can be passed as it is
+ *   rvec,tvec fp64 3 each: the pose (x_cam = R(rvec) x_world + tvec); 0 when ok is 0
+ *   mask      n x u8: 1 for the used points that are inliers, 0 elsewhere; inliers the number of ones; ok cv2's return value
+ * m == 4: the P3P pose of the four points with every point an inlier, no refinement (what OpenCV does). m < 4 (which OpenCV refuses with
+ * an assertion) and a RANSAC that finds no model give ok 0, a zero mask, inliers 0 and rvec = tvec = 0. iterations <= 0 runs one;
+ * reproj_error may be any float (it is squared; NaN finds no inlier).
+ * Errors, before anything is launched (buffers and the context's launch count untouched): HV_ERR_INVALID for a NULL context / rvec /
+ * tvec / inliers / ok, a NULL xyz / xy / mask with n > 0, n < 0, or confidence outside (0, 1) or NaN (what cv::solvePnPRansac 4.13
+ * refuses); HV_ERR_UNSUPPORTED for n above HV_PNP_MAX_POINTS, iterations above HV_PNP_MAX_ITERS, and intrinsics that are not finite or
+ * have a zero focal length. Every call is one launch (ctx's launch count + 1) whatever the data holds. The compacted points live in
+ * scratch memory of the context (120 bytes per point, shared with hv_find_essential*), which only grows. */
+#define HV_PNP_MAX_POINTS 4096
+#define HV_PNP_MAX_ITERS 4096
+int hv_solve_pnp_ransac(hv_ctx* ctx, const float* xyz, const float* xy, const uint8_t* status, int n, double fx, double fy, double cx,
+                        double cy, int iterations, float reproj_error, double confidence, double* rvec, double* tvec, uint8_t* mask,
+                        int* inliers, int* ok);                                                             /* host, synchronises */
+int hv_solve_pnp_ransac_device(hv_ctx* ctx, const float* d_xyz, const float* d_xy, const uint8_t* d_status, int n, double fx, double fy,
+                               double cx, double cy, int iterations, float reproj_error, double confidence, double* d_rvec,
+                               double* d_tvec, uint8_t* d_mask, int* d_inliers, int* d_ok);                  /* device, asynchronous */
+/* hv_solve_pnp_ransac_device for 1..HV_ESSENTIAL_BATCH_MAX jobs (one per session sharing the context) in the one launch of one call:
+ * every job's outputs are bit-identical to the per-call function's. Points, status, n, intrinsics and outputs are per job; iterations,
+ * reproj_error and confidence the batch's. Errors as hv_solve_pnp_ransac_device's for every job, and HV_ERR_INVALID for a NULL jobs array
+ * or njobs outside 1..HV_ESSENTIAL_BATCH_MAX, all before anything is launched. */
+typedef struct hv_pnp_job {
+    const float* d_xyz; const float* d_xy; const uint8_t* d_status;
+    int n;
+    double fx, fy, cx, cy;
+    double* d_rvec; double* d_tvec; uint8_t* d_mask; int* d_inliers; int* d_ok;
+} hv_pnp_job;
+int hv_solve_pnp_ransac_batch_device(hv_ctx* ctx, const hv_pnp_job* jobs, int njobs, int iterations, float reproj_error, double confidence);
+
 /* ---------------------------------------------------------------- frame ingest (SURVEY.md 8(f) N4) -------- */
 /* Device part of tracker::Image::Factory::build / buildStereo (src/tracker/image.cpp:243-308): colour -> gray
  * (accelerated-arrays pixelwiseAffine, image.cpp:360-366) and undistortion / rectification (UndistorterImplementation::undistort,
