@@ -749,7 +749,9 @@ __device__ static void pnp_l6x10(const double (*v)[12], const double (*cws)[3], 
     }
 }
 
-/* R = U V^T of the SVD of abt (3 x 3 row-major), OpenCV's last-row flip when det R < 0; u3 = u1 x u2 where sigma3 <= 1e-8 sigma1 */
+/* R = U V^T of the SVD of abt (3 x 3 row-major), OpenCV's last-row flip when det R < 0. Where sigma3 <= 1e-8 sigma1 (points on a
+ * plane) u3 is not determined by abt and is taken as det(V) (u1 x u2), so that det R = +1 and R is the nearest rotation: u1 x u2 alone
+ * gives det R = det V, and the flip of a reflection's last row is not the nearest rotation. */
 __device__ static void pnp_procrustes(const double* abt, double* R)
 {
     double A[9], V[9], w[3], U[9];
@@ -766,7 +768,10 @@ __device__ static void pnp_procrustes(const double* abt, double* R)
         const double u1[3] = {U[0], U[3], U[6]}, u2[3] = {U[1], U[4], U[7]};
         double u3[3];
         pnp_cross(u1, u2, u3);
-        U[2] = u3[0]; U[5] = u3[1]; U[8] = u3[2];
+        const double dv = ((((Vs[0] * Vs[4] * Vs[8] + Vs[1] * Vs[5] * Vs[6]) + Vs[2] * Vs[3] * Vs[7]) - Vs[2] * Vs[4] * Vs[6]) -
+                           Vs[1] * Vs[3] * Vs[8]) - Vs[0] * Vs[5] * Vs[7];
+        const double sg = dv < 0.0 ? -1.0 : 1.0;
+        U[2] = sg * u3[0]; U[5] = sg * u3[1]; U[8] = sg * u3[2];
     }
     for (int i = 0; i < 3; i++)
         for (int j = 0; j < 3; j++) R[3 * i + j] = (U[3 * i] * Vs[3 * j] + U[3 * i + 1] * Vs[3 * j + 1]) + U[3 * i + 2] * Vs[3 * j + 2];

@@ -911,7 +911,9 @@ static void l6x10(const double (*v)[12], const double (*cws)[3], double* L, doub
     }
 }
 
-/* R = U V^T of the SVD of abt (3 x 3 row-major), OpenCV's last-row flip when det R < 0; u3 = u1 x u2 where sigma3 <= 1e-8 sigma1 */
+/* R = U V^T of the SVD of abt (3 x 3 row-major), OpenCV's last-row flip when det R < 0. Where sigma3 <= 1e-8 sigma1 (points on a
+ * plane) u3 is not determined by abt and is taken as det(V) (u1 x u2), so that det R = +1 and R is the nearest rotation: u1 x u2 alone
+ * gives det R = det V, and the flip of a reflection's last row is not the nearest rotation. */
 static void procrustes(const double* abt, double* R)
 {
     double A[9], V[9], w[3], U[9];
@@ -928,13 +930,41 @@ static void procrustes(const double* abt, double* R)
         const double u1[3] = {U[0], U[3], U[6]}, u2[3] = {U[1], U[4], U[7]};
         double u3[3];
         pnp_cross(u1, u2, u3);
-        U[2] = u3[0]; U[5] = u3[1]; U[8] = u3[2];
+        const double dv = ((((Vs[0] * Vs[4] * Vs[8] + Vs[1] * Vs[5] * Vs[6]) + Vs[2] * Vs[3] * Vs[7]) - Vs[2] * Vs[4] * Vs[6]) -
+                           Vs[1] * Vs[3] * Vs[8]) - Vs[0] * Vs[5] * Vs[7];
+        const double sg = dv < 0.0 ? -1.0 : 1.0;
+        U[2] = sg * u3[0]; U[5] = sg * u3[1]; U[8] = sg * u3[2];
     }
     for (int i = 0; i < 3; i++)
         for (int j = 0; j < 3; j++) R[3 * i + j] = (U[3 * i] * Vs[3 * j] + U[3 * i + 1] * Vs[3 * j + 1]) + U[3 * i + 2] * Vs[3 * j + 2];
     const double det = ((((R[0] * R[4] * R[8] + R[1] * R[5] * R[6]) + R[2] * R[3] * R[7]) - R[2] * R[4] * R[6]) - R[1] * R[3] * R[8]) -
                        R[0] * R[5] * R[7];
     if (det < 0.0) { R[6] = -R[6]; R[7] = -R[7]; R[8] = -R[8]; }
+}
+
+/* epnp::choose_control_points: the centroid c0 (c->c0 is set to it) and c0 + sqrt(w_i / n) u_i along the principal axes */
+static void control_points(EpnpCtx* c, int n, double* c0, double (*cws)[3])
+{
+    double cov6[6], A[9], V[9], w[3];
+    pnp_reduce(3, n, term_pw, c, c0);
+    for (int k = 0; k < 3; k++) c0[k] = c0[k] / n;
+    c->c0 = c0;
+    pnp_reduce(6, n, term_cov, c, cov6);
+    for (int e = 0; e < 6; e++) { A[3 * SYM3[e][0] + SYM3[e][1]] = cov6[e]; A[3 * SYM3[e][1] + SYM3[e][0]] = cov6[e]; }
+    pnp_ocv_svd3(A, w, V);
+    for (int k = 0; k < 3; k++) cws[0][k] = c0[k];
+    for (int i = 1; i < 4; i++) {
+        const double kk = sqrt(w[i - 1] / n);
+        for (int j = 0; j < 3; j++) cws[i][j] = c0[j] + kk * V[3 * (i - 1) + j];
+    }
+}
+
+/* EPnP's four control points (4 x 3, row-major) of n world points (3 n), as orc_pnp_epnp chooses them */
+void orc_pnp_epnp_control_points(const double* pws, int n, double* cws)
+{
+    EpnpCtx c = {pws, NULL, NULL, NULL, NULL, NULL, 0.0, 0.0, 0.0, 0.0, NULL, NULL};
+    double c0[3];
+    control_points(&c, n, c0, (double (*)[3])cws);
 }
 
 /* epnp::compute_pose of n points (world pws (3 n), image us (2 n), already OpenCV's undistort round trip); R row-major, t */
@@ -944,21 +974,8 @@ void orc_pnp_epnp(const double* pws, const double* us, int n, double fu, double 
     double* pcs = (double*)malloc(sizeof(double) * 3 * (size_t)n);
     mtm_pairs();
     EpnpCtx c = {pws, us, al, pcs, NULL, NULL, fu, fv, uc, vc, NULL, NULL};
-    double c0[3], cov6[6], cws[4][3];
-    pnp_reduce(3, n, term_pw, &c, c0);
-    for (int k = 0; k < 3; k++) c0[k] = c0[k] / n;
-    c.c0 = c0;
-    pnp_reduce(6, n, term_cov, &c, cov6);
-    {
-        double A[9], V[9], w[3];
-        for (int e = 0; e < 6; e++) { A[3 * SYM3[e][0] + SYM3[e][1]] = cov6[e]; A[3 * SYM3[e][1] + SYM3[e][0]] = cov6[e]; }
-        pnp_ocv_svd3(A, w, V);
-        for (int k = 0; k < 3; k++) cws[0][k] = c0[k];
-        for (int i = 1; i < 4; i++) {
-            const double kk = sqrt(w[i - 1] / n);
-            for (int j = 0; j < 3; j++) cws[i][j] = c0[j] + kk * V[3 * (i - 1) + j];
-        }
-    }
+    double c0[3], cws[4][3];
+    control_points(&c, n, c0, cws);
     double ci[9];
     {
         double A[9], V[9], w[3];

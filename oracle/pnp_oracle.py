@@ -20,6 +20,8 @@ class OraclePnp:
         L.orc_pnp_model4.restype = _i
         L.orc_pnp_epnp.argtypes = [_vp, _vp, _i, _d, _d, _d, _d, _vp, _vp]
         L.orc_pnp_epnp.restype = None
+        L.orc_pnp_epnp_control_points.argtypes = [_vp, _i, _vp]
+        L.orc_pnp_epnp_control_points.restype = None
         L.orc_pnp_rodrigues_v2r.argtypes = [_vp, _vp]
         L.orc_pnp_rodrigues_r2v.argtypes = [_vp, _vp]
         L.orc_pnp_sincos.argtypes = [_d, _vp, _vp]
@@ -64,15 +66,23 @@ class OraclePnp:
             return None
         return mdl[:3].copy(), mdl[3:].copy()
 
-    def epnp(self, X, x, fx, fy, cx, cy):
-        """EPnP of (n, 3) world points at (n, 2) pixels (OpenCV's undistort round trip applied here): (rvec (3,), tvec (3,))."""
+    def epnp(self, X, x, fx, fy, cx, cy, rotation=False):
+        """EPnP of (n, 3) world points at (n, 2) pixels (OpenCV's undistort round trip applied here): (rvec (3,), tvec (3,)), and the
+        rotation matrix R (3, 3) that rvec is made from if `rotation`."""
         pw = np.ascontiguousarray(X, np.float64).reshape(-1, 3)
         x = np.asarray(x, np.float64).reshape(-1, 2)
         us = np.ascontiguousarray(np.c_[((x[:, 0] - cx) * (1.0 / fx)) * fx + cx, ((x[:, 1] - cy) * (1.0 / fy)) * fy + cy])
         R, t, r = np.zeros(9), np.zeros(3), np.zeros(3)
         self.lib.orc_pnp_epnp(pw.ctypes.data, us.ctypes.data, pw.shape[0], fx, fy, cx, cy, R.ctypes.data, t.ctypes.data)
         self.lib.orc_pnp_rodrigues_r2v(R.ctypes.data, r.ctypes.data)
-        return r, t
+        return (r, t, R.reshape(3, 3)) if rotation else (r, t)
+
+    def control_points(self, X):
+        """EPnP's four control points (4, 3) of (n, 3) world points: the centroid, then one along each principal axis"""
+        pw = np.ascontiguousarray(X, np.float64).reshape(-1, 3)
+        cws = np.zeros(12)
+        self.lib.orc_pnp_epnp_control_points(pw.ctypes.data, pw.shape[0], cws.ctypes.data)
+        return cws.reshape(4, 3)
 
     def rodrigues(self, v):
         """rvec (3,) -> R (3, 3), or R (3, 3) -> rvec (3,)"""
