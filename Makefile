@@ -13,7 +13,7 @@ all: $(LIB) $(DRV) oracle
 
 $(OBJ)/%.o: $(CSRC)/%.cu $(wildcard $(CSRC)/*.cuh) $(wildcard $(CSRC)/*.h) include/hybvio_b200.h
 	@mkdir -p $(OBJ)
-	$(NVCC) $(NVFLAGS) $(if $(filter lk essential pose pnp,$*),--fmad=false,) -c $< -o $@ 2> $(OBJ)/$*.ptxas.log || (cat $(OBJ)/$*.ptxas.log; false)
+	$(NVCC) $(NVFLAGS) $(if $(filter lk essential pose pnp triangulate,$*),--fmad=false,) -c $< -o $@ 2> $(OBJ)/$*.ptxas.log || (cat $(OBJ)/$*.ptxas.log; false)
 
 $(LIB): $(OBJS)
 	$(NVCC) $(ARCH) -shared -o $@ $^ -Xlinker --version-script=$(CSRC)/exports.map
@@ -27,7 +27,7 @@ TOBJ := build/obj_timing
 TLIB := hybvio_b200/libhybvio_b200_timing.so
 $(TOBJ)/%.o: $(CSRC)/%.cu $(wildcard $(CSRC)/*.cuh) $(wildcard $(CSRC)/*.h) include/hybvio_b200.h
 	@mkdir -p $(TOBJ)
-	$(NVCC) $(NVFLAGS) -DHV_EKF_TIMING $(if $(filter lk essential pose pnp,$*),--fmad=false,) -c $< -o $@ 2> $(TOBJ)/$*.ptxas.log || (cat $(TOBJ)/$*.ptxas.log; false)
+	$(NVCC) $(NVFLAGS) -DHV_EKF_TIMING $(if $(filter lk essential pose pnp triangulate,$*),--fmad=false,) -c $< -o $@ 2> $(TOBJ)/$*.ptxas.log || (cat $(TOBJ)/$*.ptxas.log; false)
 timing: $(patsubst $(CSRC)/%.cu,$(TOBJ)/%.o,$(CU))
 	$(NVCC) $(ARCH) -shared -o $(TLIB) $^ -Xlinker --version-script=$(CSRC)/exports.map
 

@@ -133,6 +133,16 @@ class PoseJob(ctypes.Structure):
                 ("d_R", c_void_p), ("d_t", c_void_p), ("d_mask_out", c_void_p), ("d_good", c_void_p)]
 
 
+class TriangulateJob(ctypes.Structure):
+    """hv_triangulate_job: one session's projection matrices, correspondences, statuses and outputs in the batched triangulation (see
+    triangulate_job)"""
+    _fields_ = [("P1", c_double * 12), ("P2", c_double * 12), ("d_xy1", c_void_p), ("d_xy2", c_void_p), ("d_status", c_void_p),
+                ("d_status2", c_void_p), ("n", c_int), ("d_X4", c_void_p), ("d_xyz", c_void_p), ("d_used", c_void_p)]
+
+
+TRIANGULATE_MAX_POINTS = 1 << 20    # HV_TRIANGULATE_MAX_POINTS
+
+
 class IngestJob(ctypes.Structure):
     """hv_ingest_job: one frame of hv_ingest_frames (see ingest_job)"""
     _fields_ = [("ing", c_void_p), ("src", c_void_p), ("stride_bytes", c_size_t), ("channels", c_int), ("coeff", c_void_p),
@@ -208,6 +218,10 @@ def load():
                                         ctypes.c_float, c_double, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
     lib.hv_solve_pnp_ransac_device.argtypes = lib.hv_solve_pnp_ransac.argtypes
     lib.hv_solve_pnp_ransac_batch_device.argtypes = [c_void_p, ctypes.POINTER(PnpJob), c_int, c_int, ctypes.c_float, c_double]
+    lib.hv_triangulate_points.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
+                                          c_void_p]
+    lib.hv_triangulate_points_device.argtypes = lib.hv_triangulate_points.argtypes
+    lib.hv_triangulate_points_batch_device.argtypes = [c_void_p, ctypes.POINTER(TriangulateJob), c_int]
     _bind_ekf(lib)
     _lib = lib
     return lib
@@ -501,6 +515,34 @@ class Context:
         check(self.lib.hv_solve_pnp_ransac_batch_device(self.h, J, len(jobs), iterations, reproj_error, confidence),
               "hv_solve_pnp_ransac_batch_device")
 
+    # ---- cv::triangulatePoints(P1, P2, xy1, xy2) + cv::convertPointsFromHomogeneous: one launch per call
+    def triangulate_points(self, P1, P2, xy1, xy2, status=None, status2=None):
+        """hv_triangulate_points on host arrays: P1, P2 (3, 4); xy1, xy2 float32 (converted) in a shape cv2.triangulatePoints takes,
+        (2, n) or (n, 1, 2), or LK's (n, 2) (a (2, 2) array is read as (2, n), as cv2 reads it); status, status2 (n,) uint8 or None.
+        Returns X4 (4, n) float32: what cv2.triangulatePoints returns for float32 points, with zero columns where a status is 0."""
+        a, b = _tri_points(xy1, "xy1"), _tri_points(xy2, "xy2")
+        if a.shape != b.shape:
+            raise ValueError(f"xy1 {np.shape(xy1)} and xy2 {np.shape(xy2)} hold different point counts")
+        n = a.shape[0]
+        st = [None if s is None else np.ascontiguousarray(s, np.uint8).reshape(-1) for s in (status, status2)]
+        if any(s is not None and s.shape != (n,) for s in st):
+            raise ValueError(f"a status does not hold {n} points")
+        X4 = np.zeros((4, n), np.float32)
+        check(self.lib.hv_triangulate_points(self.h, _ptr(_tri_P(P1)), _ptr(_tri_P(P2)), _ptr(a), _ptr(b), _ptr(st[0]), _ptr(st[1]), n,
+                                             _ptr(X4) if n else None, None, None), "hv_triangulate_points")
+        return X4
+
+    def triangulate_points_device(self, P1, P2, d_xy1, d_xy2, d_X4=None, d_xyz=None, d_used=None, d_status=None, d_status2=None, n=None):
+        """hv_triangulate_points_device on CUDA tensors (see triangulate_job for the buffers); asynchronous on the context's stream."""
+        j = triangulate_job(P1, P2, d_xy1, d_xy2, d_X4, d_xyz, d_used, d_status, d_status2, n)
+        check(self.lib.hv_triangulate_points_device(self.h, j.P1, j.P2, j.d_xy1, j.d_xy2, j.d_status, j.d_status2, j.n, j.d_X4, j.d_xyz,
+                                                    j.d_used), "hv_triangulate_points_device")
+
+    def triangulate_points_batch_device(self, jobs):
+        """hv_triangulate_points_batch_device: every job (see triangulate_job) in one launch; asynchronous."""
+        J = (TriangulateJob * len(jobs))(*jobs)
+        check(self.lib.hv_triangulate_points_batch_device(self.h, J, len(jobs)), "hv_triangulate_points_batch_device")
+
     # ---- cv::recoverPose(E, xy1, xy2, K, R, t, distance_thresh, mask): one launch per call
     def recover_pose(self, E, xy1, xy2, fx, fy, cx, cy, distance_thresh=50.0, mask=None):
         """hv_recover_pose on host arrays: E (3, 3) row-major, xy1, xy2 (n, 2) float32 (converted), mask (n,) or (n, 1) uint8 or None.
@@ -632,6 +674,43 @@ def pnp_job(d_xyz, d_xy, d_rvec, d_tvec, d_mask, d_inliers, d_ok, fx, fy, cx, cy
         raise ValueError("pnp_job: a buffer is smaller than n points (or rvec, tvec smaller than 3 doubles)")
     return PnpJob(_ptr(d_xyz), _ptr(d_xy), _ptr(d_status), n, fx, fy, cx, cy, _ptr(d_rvec), _ptr(d_tvec), _ptr(d_mask), _ptr(d_inliers),
                   _ptr(d_ok))
+
+def _tri_P(P):
+    P = np.ascontiguousarray(P, np.float64)
+    if P.shape != (3, 4):
+        raise ValueError(f"projection matrix {P.shape} is not (3, 4)")
+    return P
+
+
+def _tri_points(xy, what):
+    """(n, 2) float32 points from cv2's (2, n) or (n, 1, 2), or LK's (n, 2)"""
+    a = np.asarray(xy, np.float32)
+    if a.ndim == 3 and a.shape[1:] == (1, 2):
+        return np.ascontiguousarray(a.reshape(-1, 2))
+    if a.ndim == 2 and a.shape[0] == 2:
+        return np.ascontiguousarray(a.T)
+    if a.ndim == 2 and a.shape[1] == 2:
+        return np.ascontiguousarray(a)
+    raise ValueError(f"{what} {a.shape} is not (2, n), (n, 1, 2) or (n, 2)")
+
+
+def triangulate_job(P1, P2, d_xy1, d_xy2, d_X4=None, d_xyz=None, d_used=None, d_status=None, d_status2=None, n=None):
+    """A TriangulateJob: P1, P2 (3, 4) host arrays (copied into the job), contiguous CUDA tensors d_xy1, d_xy2 (capacity, 2) float32,
+    d_status, d_status2 (capacity,) uint8 or None, d_X4 float32 of at least 4 n (row r at r n) or None, d_xyz (capacity, 3) float32 or
+    None, d_used (capacity,) uint8 or None (may be d_status or d_status2); n: the first n points (all). The tensors must outlive the call
+    that uses the job."""
+    opt = tuple((t, s) for t, s in ((d_X4, 4), (d_xyz, 4), (d_used, 1), (d_status, 1), (d_status2, 1)) if t is not None)
+    for t, size in ((d_xy1, 4), (d_xy2, 4)) + opt:
+        if not t.is_cuda or not t.is_contiguous() or t.element_size() != size:
+            raise ValueError("triangulate_job: every buffer must be a contiguous CUDA tensor of the documented dtype")
+    cap = d_xy1.numel() // 2
+    n = cap if n is None else n
+    if (n > cap or d_xy2.numel() // 2 < n or (d_X4 is not None and d_X4.numel() < 4 * n) or (d_xyz is not None and d_xyz.numel() < 3 * n)
+            or any(t is not None and t.numel() < n for t in (d_used, d_status, d_status2))):
+        raise ValueError("triangulate_job: a buffer is smaller than n points")
+    return TriangulateJob((c_double * 12)(*_tri_P(P1).ravel()), (c_double * 12)(*_tri_P(P2).ravel()), _ptr(d_xy1), _ptr(d_xy2),
+                          _ptr(d_status), _ptr(d_status2), n, _ptr(d_X4), _ptr(d_xyz), _ptr(d_used))
+
 
 def pose_job(d_E, d_xy1, d_xy2, d_R, d_t, d_mask_out, d_good, fx, fy, cx, cy, d_nsol=None, d_mask_in=None, n=None):
     """A PoseJob on contiguous CUDA tensors: d_E float64 (at least 9: column-major, the first slot is used), d_nsol (1,) int32 or None

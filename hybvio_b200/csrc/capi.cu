@@ -1424,6 +1424,106 @@ int hv_solve_pnp_ransac_batch_device(hv_ctx* c, const hv_pnp_job* jobs, int njob
     return HV_OK;
 }
 
+// ------------------------------------------------------------------------------------------------ two-view triangulation (N3)
+// Checks one job and fills its arguments; P1 and P2 are read here, on the host, and travel by value.
+static int tri_args(const char* who, const double* P1, const double* P2, const float* xy1, const float* xy2, const uint8_t* status,
+                    const uint8_t* status2, int n, float* X4, float* xyz, uint8_t* used, TriArgs& a)
+{
+    if (!P1 || !P2) { hv_set_error("%s: NULL P1 or P2", who); return HV_ERR_INVALID; }
+    if (n < 0) { hv_set_error("%s: n = %d", who, n); return HV_ERR_INVALID; }
+    if (n > 0 && (!xy1 || !xy2)) { hv_set_error("%s: NULL xy1 or xy2", who); return HV_ERR_INVALID; }
+    if (n > 0 && !X4 && !xyz) { hv_set_error("%s: NULL X4 and xyz", who); return HV_ERR_INVALID; }
+    if (n > HV_TRIANGULATE_MAX_POINTS) { hv_set_error("%s: %d points (at most %d)", who, n, HV_TRIANGULATE_MAX_POINTS); return HV_ERR_UNSUPPORTED; }
+    for (int k = 0; k < 12; k++)
+        if (!std::isfinite(P1[k]) || !std::isfinite(P2[k])) {
+            hv_set_error("%s: P1[%d] = %g, P2[%d] = %g: not finite", who, k, P1[k], k, P2[k]);
+            return HV_ERR_UNSUPPORTED;
+        }
+    memset(&a, 0, sizeof(a));
+    memcpy(a.P1, P1, sizeof(a.P1));
+    memcpy(a.P2, P2, sizeof(a.P2));
+    a.xy1 = (const float2*)xy1; a.xy2 = (const float2*)xy2; a.status = status; a.status2 = status2; a.n = n;
+    a.X4 = X4; a.xyz = xyz; a.used = used;
+    return HV_OK;
+}
+
+int hv_triangulate_points_device(hv_ctx* c, const double* P1, const double* P2, const float* dXY1, const float* dXY2, const uint8_t* dStatus,
+                                 const uint8_t* dStatus2, int n, float* dX4, float* dXYZ, uint8_t* dUsed)
+{
+    const char* who = "hv_triangulate_points_device";
+    if (!c) { hv_set_error("%s: NULL context", who); return HV_ERR_INVALID; }
+    TriBatchArgs b;
+    memset(&b, 0, sizeof(b));
+    const int rc = tri_args(who, P1, P2, dXY1, dXY2, dStatus, dStatus2, n, dX4, dXYZ, dUsed, b.job[0]);
+    if (rc != HV_OK) return rc;
+    HV_CUDA(cudaSetDevice(c->device));
+    HV_CUDA(hv_launch_triangulate(b, 1, n, c->stream));
+    c->launches += 1;
+    return HV_OK;
+}
+
+int hv_triangulate_points(hv_ctx* c, const double* P1, const double* P2, const float* xy1, const float* xy2, const uint8_t* status,
+                          const uint8_t* status2, int n, float* X4, float* xyz, uint8_t* used)
+{
+    const char* who = "hv_triangulate_points";
+    if (!c) { hv_set_error("%s: NULL context", who); return HV_ERR_INVALID; }
+    TriBatchArgs b;
+    memset(&b, 0, sizeof(b));
+    int rc = tri_args(who, P1, P2, xy1, xy2, status, status2, n, X4, xyz, used, b.job[0]);
+    if (rc != HV_OK) return rc;
+    HV_CUDA(cudaSetDevice(c->device));
+    // staging block: [X4 16n | xyz 12n | used n] back to the host, [xy1 8n | xy2 8n | status n | status2 n] to the device
+    const size_t N = (size_t)n;
+    const size_t oXYZ = 16 * N, oUsed = oXYZ + 12 * N, oXY1 = align_up(oUsed + N, 16), oXY2 = oXY1 + 8 * N, oSt = oXY2 + 8 * N;
+    const size_t oSt2 = oSt + (status ? N : 0), total = oSt2 + (status2 ? N : 0);
+    rc = hv_ctx_reserve_stage(c, total);
+    if (rc != HV_OK) return rc;
+    uint8_t* hs = (uint8_t*)c->h_stage; uint8_t* ds = (uint8_t*)c->d_stage;
+    if (n > 0) {
+        memcpy(hs + oXY1, xy1, 8 * N);
+        memcpy(hs + oXY2, xy2, 8 * N);
+        if (status) memcpy(hs + oSt, status, N);
+        if (status2) memcpy(hs + oSt2, status2, N);
+        HV_CUDA(cudaMemcpyAsync(ds + oXY1, hs + oXY1, total - oXY1, cudaMemcpyHostToDevice, c->stream));
+    }
+    TriArgs& a = b.job[0];
+    a.xy1 = (const float2*)(ds + oXY1); a.xy2 = (const float2*)(ds + oXY2);
+    a.status = status ? ds + oSt : nullptr; a.status2 = status2 ? ds + oSt2 : nullptr;
+    a.X4 = X4 ? (float*)ds : nullptr; a.xyz = xyz ? (float*)(ds + oXYZ) : nullptr; a.used = used ? ds + oUsed : nullptr;
+    HV_CUDA(hv_launch_triangulate(b, 1, n, c->stream));
+    c->launches += 1;
+    if (n > 0) HV_CUDA(cudaMemcpyAsync(hs, ds, oUsed + N, cudaMemcpyDeviceToHost, c->stream));
+    HV_CUDA(cudaStreamSynchronize(c->stream));
+    if (n > 0) {
+        if (X4) memcpy(X4, hs, 16 * N);
+        if (xyz) memcpy(xyz, hs + oXYZ, 12 * N);
+        if (used) memcpy(used, hs + oUsed, N);
+    }
+    return HV_OK;
+}
+
+int hv_triangulate_points_batch_device(hv_ctx* c, const hv_triangulate_job* jobs, int njobs)
+{
+    const char* who = "hv_triangulate_points_batch_device";
+    if (!c || !jobs) { hv_set_error("%s: NULL context or jobs", who); return HV_ERR_INVALID; }
+    if (njobs < 1 || njobs > HV_ESSENTIAL_BATCH_MAX) { hv_set_error("%s: %d jobs (1..%d per call)", who, njobs, HV_ESSENTIAL_BATCH_MAX); return HV_ERR_INVALID; }
+    TriBatchArgs b;
+    memset(&b, 0, sizeof(b));
+    int maxn = 0;
+    for (int j = 0; j < njobs; j++) {
+        const hv_triangulate_job& J = jobs[j];
+        char w[64];
+        snprintf(w, sizeof(w), "%s job %d", who, j);
+        const int rc = tri_args(w, J.P1, J.P2, J.d_xy1, J.d_xy2, J.d_status, J.d_status2, J.n, J.d_X4, J.d_xyz, J.d_used, b.job[j]);
+        if (rc != HV_OK) return rc;
+        if (J.n > maxn) maxn = J.n;
+    }
+    HV_CUDA(cudaSetDevice(c->device));
+    HV_CUDA(hv_launch_triangulate(b, njobs, maxn, c->stream));
+    c->launches += 1;
+    return HV_OK;
+}
+
 // ------------------------------------------------------------------------------------------------ frame ingest (N4)
 struct hv_ingest {
     hv_ctx* ctx = nullptr;

@@ -286,6 +286,23 @@ struct PnpBatchArgs {
 static_assert(sizeof(PnpBatchArgs) <= HV_KERNEL_PARAM_MAX, "pnp batch arguments exceed the kernel-parameter space");
 cudaError_t hv_launch_pnp(const PnpBatchArgs& b, int njobs, cudaStream_t stream);     // one launch, one CTA per job
 
+// ---- two-view triangulation (triangulate.cu): cv::triangulatePoints + convertPointsFromHomogeneous, up to HV_ESSENTIAL_BATCH_MAX jobs
+#define HV_TRIANGULATE_MAX_POINTS (1 << 20)
+struct TriArgs {
+    double P1[12], P2[12];            // row-major 3 x 4
+    const float2* xy1; const float2* xy2;
+    const uint8_t* status; const uint8_t* status2;     // NULL: all non-zero
+    int n;
+    float* X4;                        // 4 x n (row r at X4 + r n) or NULL
+    float* xyz;                       // n x 3 or NULL
+    uint8_t* used;                    // n, 0/1, or NULL; may be status or status2
+};
+struct TriBatchArgs {
+    TriArgs job[HV_ESSENTIAL_BATCH_MAX];
+};
+static_assert(sizeof(TriBatchArgs) <= HV_KERNEL_PARAM_MAX, "triangulation batch arguments exceed the kernel-parameter space");
+cudaError_t hv_launch_triangulate(const TriBatchArgs& b, int njobs, int maxn, cudaStream_t stream);   // one launch: grid (points, jobs)
+
 // ---- frame ingest (ingest.cu)
 #define HV_REMAP_INVALID (-32768)
 struct HvRemapEntry { short x0, y0; float xfrac, yfrac; };      // 12 bytes per output pixel (hv_remap_entry of the C ABI)

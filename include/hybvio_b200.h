@@ -390,6 +390,45 @@ typedef struct hv_pnp_job {
 } hv_pnp_job;
 int hv_solve_pnp_ransac_batch_device(hv_ctx* ctx, const hv_pnp_job* jobs, int njobs, int iterations, float reproj_error, double confidence);
 
+/* ---------------------------------------------------------------- two-view triangulation (SURVEY.md 8(f) N3) -- */
+/* cv::triangulatePoints(P1, P2, xy1[used], xy2[used], X4) and cv::convertPointsFromHomogeneous(X4^T, xyz) (OCV/calib3d/src/
+ * triangulate.cpp, OCV/core/src/lapack.cpp, fundam.cpp) for float32 points: per point the 4 x 4 DLT system of both views, formed in
+ * double, and the last row of V^T of OpenCV's own Jacobi SVD of it (JacobiSVDImpl_, restated: DESIGN.md 4.14), rounded to float -- the
+ * value cv2.triangulatePoints returns for float32 points, the sign of every column included (callers test cheirality on it, Q2 Q3 > 0
+ * as recoverPose does). Feeds hv_solve_pnp_ransac_device the 3-D points of the stereo LK's tracks without a host round trip.
+ *   P1, P2    row-major 3 x 4 fp64 projection matrices, read on the host when the function is called (also by the device calls)
+ *   xy1, xy2  n x (x, y) float32, the layout the LK calls write
+ *   status, status2  n x u8 or NULL (all non-zero); a point is used where both are non-zero -- status = stereo LK's status, status2 =
+ *             temporal LK's, and used is the one status hv_solve_pnp_ransac_device needs for the pair
+ *   X4        4 x n float32, cv2's (4, N) layout (row r at X4 + r n), or NULL
+ *   xyz       n x 3 float32, the column over its w computed in float (1 / w, then three products) where |w| > FLT_EPSILON, the column
+ *             itself elsewhere (what cv::convertPointsFromHomogeneous does), or NULL; not both X4 and xyz NULL when n > 0
+ *   used      n x u8 or NULL: 1 where the point is used, 0 elsewhere; may be status or status2
+ * An unused point gets a zero column of X4, zero xyz and used 0, so a chain never reads stale values. No cheirality or depth filter is
+ * applied: the caller's policy reads X4 or xyz.
+ * Errors, before anything is launched (buffers and the context's launch count untouched): HV_ERR_INVALID for a NULL context / P1 / P2,
+ * a NULL xy1 / xy2 with n > 0, X4 and xyz both NULL with n > 0, n < 0; HV_ERR_UNSUPPORTED for n above HV_TRIANGULATE_MAX_POINTS and a
+ * P1 or P2 with a non-finite entry (which OpenCV accepts, returning NaN). Every accepted call is one launch (ctx's launch count + 1)
+ * whatever the data holds, n = 0 included. */
+#define HV_TRIANGULATE_MAX_POINTS (1 << 20)
+int hv_triangulate_points(hv_ctx* ctx, const double* P1, const double* P2, const float* xy1, const float* xy2,
+                          const uint8_t* status, const uint8_t* status2, int n,
+                          float* X4, float* xyz, uint8_t* used);                                 /* host, synchronises */
+int hv_triangulate_points_device(hv_ctx* ctx, const double* P1, const double* P2, const float* d_xy1, const float* d_xy2,
+                                 const uint8_t* d_status, const uint8_t* d_status2, int n,
+                                 float* d_X4, float* d_xyz, uint8_t* d_used);                    /* device, asynchronous */
+/* hv_triangulate_points_device for 1..HV_ESSENTIAL_BATCH_MAX jobs (one per session sharing the context; P1 and P2 per job, since
+ * sessions have their own calibrations) in the one launch of one call: every job's outputs are bit-identical to the per-call function's.
+ * Errors as hv_triangulate_points_device's for every job, and HV_ERR_INVALID for a NULL jobs array or njobs outside
+ * 1..HV_ESSENTIAL_BATCH_MAX, all before anything is launched. */
+typedef struct hv_triangulate_job {
+    double P1[12], P2[12];
+    const float* d_xy1; const float* d_xy2; const uint8_t* d_status; const uint8_t* d_status2;
+    int n;
+    float* d_X4; float* d_xyz; uint8_t* d_used;
+} hv_triangulate_job;
+int hv_triangulate_points_batch_device(hv_ctx* ctx, const hv_triangulate_job* jobs, int njobs);
+
 /* ---------------------------------------------------------------- frame ingest (SURVEY.md 8(f) N4) -------- */
 /* Device part of tracker::Image::Factory::build / buildStereo (src/tracker/image.cpp:243-308): colour -> gray
  * (accelerated-arrays pixelwiseAffine, image.cpp:360-366) and undistortion / rectification (UndistorterImplementation::undistort,
