@@ -1,6 +1,7 @@
 // hybvio_b200/csrc/capi.cu -- C ABI (include/hybvio_b200.h): context, image pyramid, Lucas-Kanade.
 // The EKF entry points live in ekf_capi.cu.
 #include "capi_internal.h"
+#include <cassert>
 #include <climits>
 #include <cmath>
 #include <cstdarg>
@@ -76,10 +77,7 @@ int hv_ctx_destroy(hv_ctx* c)
     if (c->d_stage) cudaFree(c->d_stage);
     if (c->h_stage) cudaFreeHost(c->h_stage);
     if (c->d_done) cudaFree(c->d_done);
-    if (c->d_selectScratch) cudaFree(c->d_selectScratch);
-    if (c->d_fastScratch) cudaFree(c->d_fastScratch);
-    if (c->d_gfScratch) cudaFree(c->d_gfScratch);
-    if (c->d_essScratch) cudaFree(c->d_essScratch);
+    if (c->d_scratch) cudaFree(c->d_scratch);
     if (c->d_ekfStage) cudaFree(c->d_ekfStage);
     for (int i = 0; i < HV_EKF_STAGES; i++) {
         if (c->h_ekfStage[i]) cudaFreeHost(c->h_ekfStage[i]);
@@ -139,9 +137,80 @@ static int done_wait(hv_ctx* c, const HvDoneSignal& d, const char* who)
     return rc;
 }
 
-// ------------------------------------------------------------------------------------------------ pyramid
+// Grows the context's scratch (hv_ctx::d_scratch) to at least `bytes`, after the work that may still read it.
+static int ctx_scratch(hv_ctx* c, size_t bytes)
+{
+    if (bytes <= c->scratchBytes) return HV_OK;
+    if (c->d_scratch) { HV_CUDA(cudaStreamSynchronize(c->stream)); cudaFree(c->d_scratch); }
+    c->d_scratch = nullptr; c->scratchBytes = 0;
+    size_t cap = 1 << 16; while (cap < bytes) cap *= 2;
+    HV_CUDA(cudaMalloc(&c->d_scratch, cap));
+    c->scratchBytes = cap;
+    return HV_OK;
+}
+
 static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
+// The trip of a host-buffer call's buffers through the context's stage. The call declares each part by the field of its launch arguments
+// that holds the caller's host pointer: out() for a result, in() for an argument. send() lays the parts out (the results first, the
+// arguments behind them, every part 16-byte aligned), copies the arguments in with one H2D copy and points each field at its part's
+// device address. After the launch, recv() copies the results back with one D2H copy and one stream synchronisation. A NULL field (an
+// absent optional part) takes no space and stays NULL.
+class HostStage {
+public:
+    template <class T> void out(T*& field, size_t bytes) { add(field, bytes, true, &field, &point<T>); }
+    template <class T> void in(T*& field, size_t bytes) { add(field, bytes, false, &field, &point<T>); }
+
+    int send(hv_ctx* c)
+    {
+        size_t end = 0;
+        auto lay = [&](bool result) {
+            for (int i = 0; i < n_; i++)
+                if (p_[i].result == result && p_[i].host) { p_[i].off = align_up(end, 16); end = p_[i].off + p_[i].bytes; }
+        };
+        lay(true);
+        resultEnd_ = end;
+        const size_t argBegin = align_up(end, 16);
+        lay(false);
+        HV_CUDA(cudaSetDevice(c->device));
+        const int rc = hv_ctx_reserve_stage(c, end);
+        if (rc != HV_OK) return rc;
+        uint8_t* hs = (uint8_t*)c->h_stage; uint8_t* ds = (uint8_t*)c->d_stage;
+        for (int i = 0; i < n_; i++) {
+            const Part& p = p_[i];
+            if (!p.host) continue;
+            if (!p.result && p.bytes) memcpy(hs + p.off, p.host, p.bytes);
+            p.set(p.field, ds + p.off);
+        }
+        if (end > argBegin) HV_CUDA(cudaMemcpyAsync(ds + argBegin, hs + argBegin, end - argBegin, cudaMemcpyHostToDevice, c->stream));
+        return HV_OK;
+    }
+
+    int recv(hv_ctx* c)
+    {
+        uint8_t* hs = (uint8_t*)c->h_stage;
+        if (resultEnd_ > 0) HV_CUDA(cudaMemcpyAsync(hs, c->d_stage, resultEnd_, cudaMemcpyDeviceToHost, c->stream));
+        HV_CUDA(cudaStreamSynchronize(c->stream));
+        for (int i = 0; i < n_; i++)
+            if (p_[i].result && p_[i].host && p_[i].bytes) memcpy(const_cast<void*>(p_[i].host), hs + p_[i].off, p_[i].bytes);
+        return HV_OK;
+    }
+
+private:
+    struct Part { const void* host; size_t bytes; bool result; void* field; void (*set)(void* field, uint8_t* at); size_t off; };
+    template <class T> static void point(void* field, uint8_t* at) { *(T**)field = (T*)at; }
+    void add(const void* host, size_t bytes, bool result, void* field, void (*set)(void*, uint8_t*))
+    {
+        assert(n_ < MAX_PARTS);
+        p_[n_++] = Part{host, bytes, result, field, set, 0};
+    }
+    static const int MAX_PARTS = 8;        // hv_recover_pose and hv_solve_pnp_ransac have 8
+    Part p_[MAX_PARTS];
+    int n_ = 0;
+    size_t resultEnd_ = 0;
+};
+
+// ------------------------------------------------------------------------------------------------ pyramid
 extern "C" {
 
 int hv_pyr_create(hv_ctx* c, int w, int h, int win, int maxLevel, hv_pyr** out)
@@ -542,20 +611,14 @@ int hv_gftt_corners(hv_ctx* c, hv_pyr* pyr, int blockSize, int cell, float minRe
     if (nkp > 0) {
         HV_CUDA(cudaSetDevice(c->device));
         // device scratch: [key points 3 nkp | previous corners 2 nprev] floats; the key points never leave the device
-        const size_t scratch = sizeof(float) * (3 * (size_t)nkp + 2 * (size_t)nprev);
-        if (scratch > c->selectScratchBytes) {
-            if (c->d_selectScratch) { HV_CUDA(cudaStreamSynchronize(c->stream)); cudaFree(c->d_selectScratch); }
-            c->d_selectScratch = nullptr; c->selectScratchBytes = 0;
-            size_t cap = 4096; while (cap < scratch) cap *= 2;
-            HV_CUDA(cudaMalloc(&c->d_selectScratch, cap));
-            c->selectScratchBytes = cap;
-        }
+        rc = ctx_scratch(c, sizeof(float) * (3 * (size_t)nkp + 2 * (size_t)nprev));
+        if (rc != HV_OK) return rc;
         // staging block: [previous corners 8 nprev | count (16 bytes) | corners 8 need]
         const size_t oCount = (8 * (size_t)nprev + 15) / 16 * 16, oCorners = oCount + 16, total = oCorners + 8 * (size_t)need;
         rc = hv_ctx_reserve_stage(c, total);
         if (rc != HV_OK) return rc;
         uint8_t* hs = (uint8_t*)c->h_stage; uint8_t* hd = (uint8_t*)c->hd_stage;
-        float* dKp = c->d_selectScratch;
+        float* dKp = (float*)c->d_scratch;
         if (nprev > 0) {
             memcpy(hs, prevXY, 8 * (size_t)nprev);
             HV_CUDA(cudaMemcpyAsync(dKp + 3 * (size_t)nkp, hs, 8 * (size_t)nprev, cudaMemcpyHostToDevice, c->stream));
@@ -671,18 +734,18 @@ int hv_subpix_refine(hv_ctx* c, hv_pyr* pyr, float* xy, int n, int hw, int hh, i
 // ------------------------------------------------------------------------------------------------ the corner step of many sessions (N2)
 // Each call checks every job with the checks of the per-session call and refuses before anything is launched; then one launch on the
 // context's stream does what the per-session calls would do for every job, bit for bit. The argument blocks travel as kernel parameters.
-static_assert(HV_CORNER_BATCH_MAX == 64, "batch size of the header and of the kernels");
 
-static int corner_batch_check(const char* who, hv_ctx* c, const void* jobs, int njobs)
+// the context and job count of a batch call (the corner step's and the two-view geometry's)
+static int batch_check(const char* who, hv_ctx* c, const void* jobs, int njobs, int max)
 {
     if (!c || !jobs) { hv_set_error("%s: NULL context or jobs", who); return HV_ERR_INVALID; }
-    if (njobs < 1 || njobs > HV_CORNER_BATCH_MAX) { hv_set_error("%s: %d jobs (1..%d per call)", who, njobs, HV_CORNER_BATCH_MAX); return HV_ERR_INVALID; }
+    if (njobs < 1 || njobs > max) { hv_set_error("%s: %d jobs (1..%d per call)", who, njobs, max); return HV_ERR_INVALID; }
     return HV_OK;
 }
 
 int hv_gftt_detect_batch_device(hv_ctx* c, const hv_corner_job* jobs, int njobs, int blockSize, int cell, float minResponse)
 {
-    int rc = corner_batch_check("hv_gftt_detect_batch_device", c, jobs, njobs);
+    int rc = batch_check("hv_gftt_detect_batch_device", c, jobs, njobs, HV_CORNER_BATCH_MAX);
     if (rc != HV_OK) return rc;
     GfttBatchArgs b;
     memset(&b, 0, sizeof(b));
@@ -709,7 +772,7 @@ int hv_gftt_detect_batch_device(hv_ctx* c, const hv_corner_job* jobs, int njobs,
 
 int hv_gftt_select_batch_device(hv_ctx* c, const hv_corner_job* jobs, int njobs)
 {
-    int rc = corner_batch_check("hv_gftt_select_batch_device", c, jobs, njobs);
+    int rc = batch_check("hv_gftt_select_batch_device", c, jobs, njobs, HV_CORNER_BATCH_MAX);
     if (rc != HV_OK) return rc;
     GfttSelectBatchArgs b;
     memset(&b, 0, sizeof(b));
@@ -738,7 +801,7 @@ int hv_gftt_select_batch_device(hv_ctx* c, const hv_corner_job* jobs, int njobs)
 int hv_subpix_refine_batch_device(hv_ctx* c, const hv_subpix_job* jobs, int njobs, int hw, int hh, int zw, int zh, int criteriaType,
                                   int maxCount, double epsilon)
 {
-    int rc = corner_batch_check("hv_subpix_refine_batch_device", c, jobs, njobs);
+    int rc = batch_check("hv_subpix_refine_batch_device", c, jobs, njobs, HV_CORNER_BATCH_MAX);
     if (rc != HV_OK) return rc;
     SubpixBatchArgs b;
     memset(&b, 0, sizeof(b));
@@ -783,19 +846,14 @@ static int fast_args(const char* who, hv_ctx* c, hv_pyr* pyr, int threshold, int
     return HV_OK;
 }
 
-// points the jobs' masks and tile counts into the context's FAST scratch, grown (after the work that may still read it) as needed
+// points the jobs' masks and tile counts into the context's scratch
 static int fast_scratch(hv_ctx* c, FastArgs* jobs, const size_t* bytes, int njobs)
 {
     size_t total = 0;
     for (int j = 0; j < njobs; j++) total += bytes[j];
-    if (total > c->fastScratchBytes) {
-        if (c->d_fastScratch) { HV_CUDA(cudaStreamSynchronize(c->stream)); cudaFree(c->d_fastScratch); }
-        c->d_fastScratch = nullptr; c->fastScratchBytes = 0;
-        size_t cap = 65536; while (cap < total) cap *= 2;
-        HV_CUDA(cudaMalloc(&c->d_fastScratch, cap));
-        c->fastScratchBytes = cap;
-    }
-    uint8_t* p = (uint8_t*)c->d_fastScratch;
+    const int rc = ctx_scratch(c, total);
+    if (rc != HV_OK) return rc;
+    uint8_t* p = (uint8_t*)c->d_scratch;
     for (int j = 0; j < njobs; j++) {
         FastArgs& a = jobs[j];
         a.mask = (unsigned*)p;
@@ -805,18 +863,23 @@ static int fast_scratch(hv_ctx* c, FastArgs* jobs, const size_t* bytes, int njob
     return HV_OK;
 }
 
-int hv_fast_detect_device(hv_ctx* c, hv_pyr* pyr, int threshold, int nonmax, float* dXY, float* dResponse, int capacity, int* dCount)
+// the two launches of one checked job (hv_fast_detect, hv_fast_detect_device)
+static int fast_run(hv_ctx* c, FastArgs& a, size_t bytes)
 {
-    FastArgs a;
-    size_t bytes = 0;
-    int rc = fast_args("hv_fast_detect_device", c, pyr, threshold, nonmax, dXY, dResponse, capacity, dCount, a, &bytes);
-    if (rc != HV_OK) return rc;
     HV_CUDA(cudaSetDevice(c->device));
-    rc = fast_scratch(c, &a, &bytes, 1);
+    const int rc = fast_scratch(c, &a, &bytes, 1);
     if (rc != HV_OK) return rc;
     HV_CUDA(hv_launch_fast(a, c->stream));
     c->launches += 2;
     return HV_OK;
+}
+
+int hv_fast_detect_device(hv_ctx* c, hv_pyr* pyr, int threshold, int nonmax, float* dXY, float* dResponse, int capacity, int* dCount)
+{
+    FastArgs a;
+    size_t bytes = 0;
+    const int rc = fast_args("hv_fast_detect_device", c, pyr, threshold, nonmax, dXY, dResponse, capacity, dCount, a, &bytes);
+    return rc != HV_OK ? rc : fast_run(c, a, bytes);
 }
 
 int hv_fast_detect(hv_ctx* c, hv_pyr* pyr, int threshold, int nonmax, float* xy, float* response, int capacity, int* count)
@@ -825,28 +888,16 @@ int hv_fast_detect(hv_ctx* c, hv_pyr* pyr, int threshold, int nonmax, float* xy,
     size_t bytes = 0;
     int rc = fast_args("hv_fast_detect", c, pyr, threshold, nonmax, xy, response, capacity, count, a, &bytes);
     if (rc != HV_OK) return rc;
-    HV_CUDA(cudaSetDevice(c->device));
-    rc = fast_scratch(c, &a, &bytes, 1);
-    if (rc != HV_OK) return rc;
-    // staging block: [count (16 bytes) | xy 8 capacity | response 4 capacity]
-    const size_t oXY = 16, oResp = oXY + 8 * (size_t)capacity, total = oResp + (response ? 4 * (size_t)capacity : 0);
-    rc = hv_ctx_reserve_stage(c, total);
-    if (rc != HV_OK) return rc;
-    uint8_t* hs = (uint8_t*)c->h_stage; uint8_t* ds = (uint8_t*)c->d_stage;
-    a.count = (int*)ds; a.xy = (float2*)(ds + oXY); a.response = response ? (float*)(ds + oResp) : nullptr;
-    HV_CUDA(hv_launch_fast(a, c->stream));
-    c->launches += 2;
-    HV_CUDA(cudaMemcpyAsync(hs, ds, total, cudaMemcpyDeviceToHost, c->stream));
-    HV_CUDA(cudaStreamSynchronize(c->stream));
-    memcpy(count, hs, sizeof(int));
-    if (capacity > 0) memcpy(xy, hs + oXY, 8 * (size_t)capacity);
-    if (response && capacity > 0) memcpy(response, hs + oResp, 4 * (size_t)capacity);
-    return HV_OK;
+    HostStage s;
+    s.out(a.count, sizeof(int)); s.out(a.xy, 8 * (size_t)capacity); s.out(a.response, 4 * (size_t)capacity);
+    rc = s.send(c);
+    if (rc == HV_OK) rc = fast_run(c, a, bytes);
+    return rc != HV_OK ? rc : s.recv(c);
 }
 
 int hv_fast_detect_batch_device(hv_ctx* c, const hv_fast_job* jobs, int njobs, int threshold, int nonmax)
 {
-    int rc = corner_batch_check("hv_fast_detect_batch_device", c, jobs, njobs);
+    int rc = batch_check("hv_fast_detect_batch_device", c, jobs, njobs, HV_CORNER_BATCH_MAX);
     if (rc != HV_OK) return rc;
     FastBatchArgs b;
     memset(&b, 0, sizeof(b));
@@ -924,20 +975,15 @@ static int gf_args(const char* who, hv_ctx* c, hv_pyr* pyr, int blockSize, int m
     return HV_OK;
 }
 
-// points the jobs' words, maps, keys and grids into the context's scratch, grown (after the work that may still read it) as needed
+// points the jobs' words, maps, keys and grids into the context's scratch
 static int gf_scratch(hv_ctx* c, GoodFeaturesArgs* jobs, const size_t* bytes, int njobs)
 {
     size_t total = GF_WORDS;
     for (int j = 0; j < njobs; j++) total += bytes[j];
-    if (total > c->gfScratchBytes) {
-        if (c->d_gfScratch) { HV_CUDA(cudaStreamSynchronize(c->stream)); cudaFree(c->d_gfScratch); }
-        c->d_gfScratch = nullptr; c->gfScratchBytes = 0;
-        size_t cap = 1 << 20; while (cap < total) cap *= 2;
-        HV_CUDA(cudaMalloc(&c->d_gfScratch, cap));
-        c->gfScratchBytes = cap;
-    }
-    HV_CUDA(cudaMemsetAsync(c->d_gfScratch, 0, 2 * sizeof(unsigned) * (size_t)njobs, c->stream));
-    uint8_t* p = (uint8_t*)c->d_gfScratch;
+    const int rc = ctx_scratch(c, total);
+    if (rc != HV_OK) return rc;
+    HV_CUDA(cudaMemsetAsync(c->d_scratch, 0, 2 * sizeof(unsigned) * (size_t)njobs, c->stream));
+    uint8_t* p = (uint8_t*)c->d_scratch;
     unsigned* words = (unsigned*)p;
     p += GF_WORDS;
     for (int j = 0; j < njobs; j++) {
@@ -954,20 +1000,25 @@ static int gf_scratch(hv_ctx* c, GoodFeaturesArgs* jobs, const size_t* bytes, in
     return HV_OK;
 }
 
+// the three launches of one checked job (hv_good_features, hv_good_features_device)
+static int gf_run(hv_ctx* c, GoodFeaturesArgs& a, size_t bytes)
+{
+    HV_CUDA(cudaSetDevice(c->device));
+    const int rc = gf_scratch(c, &a, &bytes, 1);
+    if (rc != HV_OK) return rc;
+    HV_CUDA(hv_launch_good_features(a, c->stream));
+    c->launches += 3;
+    return HV_OK;
+}
+
 int hv_good_features_device(hv_ctx* c, hv_pyr* pyr, int blockSize, int maxCorners, double quality, double minDistance,
                             const uint8_t* dMask, size_t maskStride, float* dXY, float* dResponse, int capacity, int* dCount)
 {
     GoodFeaturesArgs a;
     size_t bytes = 0;
-    int rc = gf_args("hv_good_features_device", c, pyr, blockSize, maxCorners, quality, minDistance, dMask, maskStride, dXY, dResponse,
-                     capacity, dCount, a, &bytes);
-    if (rc != HV_OK) return rc;
-    HV_CUDA(cudaSetDevice(c->device));
-    rc = gf_scratch(c, &a, &bytes, 1);
-    if (rc != HV_OK) return rc;
-    HV_CUDA(hv_launch_good_features(a, c->stream));
-    c->launches += 3;
-    return HV_OK;
+    const int rc = gf_args("hv_good_features_device", c, pyr, blockSize, maxCorners, quality, minDistance, dMask, maskStride, dXY, dResponse,
+                           capacity, dCount, a, &bytes);
+    return rc != HV_OK ? rc : gf_run(c, a, bytes);
 }
 
 int hv_good_features(hv_ctx* c, hv_pyr* pyr, int blockSize, int maxCorners, double quality, double minDistance, const uint8_t* mask,
@@ -978,34 +1029,17 @@ int hv_good_features(hv_ctx* c, hv_pyr* pyr, int blockSize, int maxCorners, doub
     int rc = gf_args("hv_good_features", c, pyr, blockSize, maxCorners, quality, minDistance, mask, maskStride, xy, response, capacity,
                      count, a, &bytes);
     if (rc != HV_OK) return rc;
-    HV_CUDA(cudaSetDevice(c->device));
-    rc = gf_scratch(c, &a, &bytes, 1);
-    if (rc != HV_OK) return rc;
-    // staging block: [count (16 bytes) | xy 8 capacity | response 4 capacity | mask]
-    const size_t oXY = 16, oResp = oXY + 8 * (size_t)capacity, oMask = align_up(oResp + (response ? 4 * (size_t)capacity : 0), 16);
-    const size_t maskBytes = mask ? maskStride * (size_t)(a.h - 1) + (size_t)a.w : 0;
-    rc = hv_ctx_reserve_stage(c, oMask + maskBytes);
-    if (rc != HV_OK) return rc;
-    uint8_t* hs = (uint8_t*)c->h_stage; uint8_t* ds = (uint8_t*)c->d_stage;
-    if (mask) {
-        memcpy(hs + oMask, mask, maskBytes);
-        HV_CUDA(cudaMemcpyAsync(ds + oMask, hs + oMask, maskBytes, cudaMemcpyHostToDevice, c->stream));
-        a.mask = ds + oMask;
-    }
-    a.count = (int*)ds; a.xy = (float2*)(ds + oXY); a.response = response ? (float*)(ds + oResp) : nullptr;
-    HV_CUDA(hv_launch_good_features(a, c->stream));
-    c->launches += 3;
-    HV_CUDA(cudaMemcpyAsync(hs, ds, oMask, cudaMemcpyDeviceToHost, c->stream));
-    HV_CUDA(cudaStreamSynchronize(c->stream));
-    memcpy(count, hs, sizeof(int));
-    memcpy(xy, hs + oXY, 8 * (size_t)capacity);
-    if (response) memcpy(response, hs + oResp, 4 * (size_t)capacity);
-    return HV_OK;
+    HostStage s;
+    s.out(a.count, sizeof(int)); s.out(a.xy, 8 * (size_t)capacity); s.out(a.response, 4 * (size_t)capacity);
+    s.in(a.mask, maskStride * (size_t)(a.h - 1) + (size_t)a.w);
+    rc = s.send(c);
+    if (rc == HV_OK) rc = gf_run(c, a, bytes);
+    return rc != HV_OK ? rc : s.recv(c);
 }
 
 int hv_good_features_batch_device(hv_ctx* c, const hv_good_features_job* jobs, int njobs, int blockSize, double quality, double minDistance)
 {
-    int rc = corner_batch_check("hv_good_features_batch_device", c, jobs, njobs);
+    int rc = batch_check("hv_good_features_batch_device", c, jobs, njobs, HV_CORNER_BATCH_MAX);
     if (rc != HV_OK) return rc;
     GoodFeaturesBatchArgs b;
     memset(&b, 0, sizeof(b));
@@ -1032,20 +1066,33 @@ int hv_good_features_batch_device(hv_ctx* c, const hv_good_features_job* jobs, i
     return HV_OK;
 }
 
+// ------------------------------------------------------------------------------------------------ two-view geometry (N3)
+// Refuses a camera matrix that is not finite or has a zero focal length, and also when `refuse` holds.
+static int intrinsics_check(const char* who, double fx, double fy, double cx, double cy, bool refuse = false)
+{
+    if (refuse || !std::isfinite(fx) || !std::isfinite(fy) || !std::isfinite(cx) || !std::isfinite(cy) || fx == 0.0 || fy == 0.0) {
+        hv_set_error("%s: intrinsics (%g, %g, %g, %g) not finite or a zero focal length", who, fx, fy, cx, cy);
+        return HV_ERR_UNSUPPORTED;
+    }
+    return HV_OK;
+}
+
 // ------------------------------------------------------------------------------------------------ essential-matrix RANSAC (N3)
 // The parameters of the batch: refused as cv::findEssentialMat 4.13 refuses them (prob outside (0, 1), NaN included), or as the device
-// cannot run them (more than HV_ESSENTIAL_MAX_ITERS iterations; maxIters <= 0 runs one, as OpenCV does).
-static int ess_params(const char* who, double prob, int maxIters)
+// cannot run them (more than HV_ESSENTIAL_MAX_ITERS iterations; maxIters <= 0 runs one, as OpenCV does). Accepted, they start b.
+static int ess_params(const char* who, double prob, double threshold, int maxIters, EssentialBatchArgs& b)
 {
     if (!(prob > 0.0 && prob < 1.0)) { hv_set_error("%s: prob %g outside (0, 1)", who, prob); return HV_ERR_INVALID; }
     if (maxIters > HV_ESSENTIAL_MAX_ITERS) {
         hv_set_error("%s: max_iters %d above %d", who, maxIters, HV_ESSENTIAL_MAX_ITERS);
         return HV_ERR_UNSUPPORTED;
     }
+    memset(&b, 0, sizeof(b));
+    b.prob = prob; b.threshold = threshold; b.maxIters = maxIters;
     return HV_OK;
 }
 
-// Checks one job and fills everything but the scratch.
+// Checks one job and fills everything but the scratch; fx + fy == 0 is refused too: the threshold is divided by (fx + fy) / 2.
 static int ess_args(const char* who, const float* xy1, const float* xy2, const uint8_t* status, int n, double fx, double fy, double cx,
                     double cy, double* E, int* nsol, uint8_t* mask, int* inliers, EssentialArgs& a)
 {
@@ -1053,10 +1100,8 @@ static int ess_args(const char* who, const float* xy1, const float* xy2, const u
     if (n < 0) { hv_set_error("%s: n = %d", who, n); return HV_ERR_INVALID; }
     if (n > 0 && (!xy1 || !xy2 || !mask)) { hv_set_error("%s: NULL xy1, xy2 or mask", who); return HV_ERR_INVALID; }
     if (n > HV_ESSENTIAL_MAX_POINTS) { hv_set_error("%s: %d points (at most %d)", who, n, HV_ESSENTIAL_MAX_POINTS); return HV_ERR_UNSUPPORTED; }
-    if (!std::isfinite(fx) || !std::isfinite(fy) || !std::isfinite(cx) || !std::isfinite(cy) || fx == 0.0 || fy == 0.0 || fx + fy == 0.0) {
-        hv_set_error("%s: intrinsics (%g, %g, %g, %g) not finite or a zero focal length", who, fx, fy, cx, cy);
-        return HV_ERR_UNSUPPORTED;
-    }
+    const int rc = intrinsics_check(who, fx, fy, cx, cy, fx + fy == 0.0);
+    if (rc != HV_OK) return rc;
     memset(&a, 0, sizeof(a));
     a.xy1 = (const float2*)xy1; a.xy2 = (const float2*)xy2; a.status = status; a.n = n;
     a.fx = fx; a.fy = fy; a.cx = cx; a.cy = cy;
@@ -1064,31 +1109,29 @@ static int ess_args(const char* who, const float* xy1, const float* xy2, const u
     return HV_OK;
 }
 
-// grows the context's scratch (hv_find_essential*, hv_solve_pnp_ransac*) to `total` bytes, after the work that may still read it
-static int ctx_scratch(hv_ctx* c, size_t total)
-{
-    if (total > c->essScratchBytes) {
-        if (c->d_essScratch) { HV_CUDA(cudaStreamSynchronize(c->stream)); cudaFree(c->d_essScratch); }
-        c->d_essScratch = nullptr; c->essScratchBytes = 0;
-        size_t cap = 1 << 16; while (cap < total) cap *= 2;
-        HV_CUDA(cudaMalloc(&c->d_essScratch, cap));
-        c->essScratchBytes = cap;
-    }
-    return HV_OK;
-}
-
-// points the jobs' normalised points and indices into the context's scratch, grown as needed
+// points the jobs' normalised points and indices into the context's scratch
 static int ess_scratch(hv_ctx* c, EssentialArgs* jobs, int njobs)
 {
     size_t total = 0;
     for (int j = 0; j < njobs; j++) total += align_up(32 * (size_t)jobs[j].n, 256) + align_up(4 * (size_t)jobs[j].n, 256);
     const int rc = ctx_scratch(c, total);
     if (rc != HV_OK) return rc;
-    uint8_t* p = (uint8_t*)c->d_essScratch;
+    uint8_t* p = (uint8_t*)c->d_scratch;
     for (int j = 0; j < njobs; j++) {
         jobs[j].q = (double*)p; p += align_up(32 * (size_t)jobs[j].n, 256);
         jobs[j].idx = (int*)p; p += align_up(4 * (size_t)jobs[j].n, 256);
     }
+    return HV_OK;
+}
+
+// the launch of b's first njobs jobs, checked (every hv_find_essential* call)
+static int ess_run(hv_ctx* c, EssentialBatchArgs& b, int njobs)
+{
+    HV_CUDA(cudaSetDevice(c->device));
+    const int rc = ess_scratch(c, b.job, njobs);
+    if (rc != HV_OK) return rc;
+    HV_CUDA(hv_launch_essential(b, njobs, c->stream));
+    c->launches += 1;
     return HV_OK;
 }
 
@@ -1098,19 +1141,10 @@ int hv_find_essential_device(hv_ctx* c, const float* dXY1, const float* dXY2, co
 {
     const char* who = "hv_find_essential_device";
     if (!c) { hv_set_error("%s: NULL context", who); return HV_ERR_INVALID; }
-    int rc = ess_params(who, prob, maxIters);
-    if (rc != HV_OK) return rc;
     EssentialBatchArgs b;
-    memset(&b, 0, sizeof(b));
-    rc = ess_args(who, dXY1, dXY2, dStatus, n, fx, fy, cx, cy, dE, dNsol, dMask, dInliers, b.job[0]);
-    if (rc != HV_OK) return rc;
-    b.prob = prob; b.threshold = threshold; b.maxIters = maxIters;
-    HV_CUDA(cudaSetDevice(c->device));
-    rc = ess_scratch(c, b.job, 1);
-    if (rc != HV_OK) return rc;
-    HV_CUDA(hv_launch_essential(b, 1, c->stream));
-    c->launches += 1;
-    return HV_OK;
+    int rc = ess_params(who, prob, threshold, maxIters, b);
+    if (rc == HV_OK) rc = ess_args(who, dXY1, dXY2, dStatus, n, fx, fy, cx, cy, dE, dNsol, dMask, dInliers, b.job[0]);
+    return rc != HV_OK ? rc : ess_run(c, b, 1);
 }
 
 int hv_find_essential(hv_ctx* c, const float* xy1, const float* xy2, const uint8_t* status, int n, double fx, double fy, double cx,
@@ -1118,51 +1152,27 @@ int hv_find_essential(hv_ctx* c, const float* xy1, const float* xy2, const uint8
 {
     const char* who = "hv_find_essential";
     if (!c) { hv_set_error("%s: NULL context", who); return HV_ERR_INVALID; }
-    int rc = ess_params(who, prob, maxIters);
-    if (rc != HV_OK) return rc;
     EssentialBatchArgs b;
-    memset(&b, 0, sizeof(b));
-    rc = ess_args(who, xy1, xy2, status, n, fx, fy, cx, cy, E, nsol, mask, inliers, b.job[0]);
+    int rc = ess_params(who, prob, threshold, maxIters, b);
+    if (rc == HV_OK) rc = ess_args(who, xy1, xy2, status, n, fx, fy, cx, cy, E, nsol, mask, inliers, b.job[0]);
     if (rc != HV_OK) return rc;
-    b.prob = prob; b.threshold = threshold; b.maxIters = maxIters;
-    HV_CUDA(cudaSetDevice(c->device));
-    rc = ess_scratch(c, b.job, 1);
-    if (rc != HV_OK) return rc;
-    // staging block: [E 80 doubles | nsol, inliers | mask n] back to the host, [xy1 8n | xy2 8n | status n] to the device
-    const size_t oMask = 8 * 90 + 16, oXY1 = align_up(oMask + (size_t)n, 16);
-    const size_t oXY2 = oXY1 + 8 * (size_t)n, oSt = oXY2 + 8 * (size_t)n, total = oSt + (status ? (size_t)n : 0);
-    rc = hv_ctx_reserve_stage(c, total);
-    if (rc != HV_OK) return rc;
-    uint8_t* hs = (uint8_t*)c->h_stage; uint8_t* ds = (uint8_t*)c->d_stage;
-    if (n > 0) {
-        memcpy(hs + oXY1, xy1, 8 * (size_t)n);
-        memcpy(hs + oXY2, xy2, 8 * (size_t)n);
-        if (status) memcpy(hs + oSt, status, (size_t)n);
-    }
-    if (total > oXY1) HV_CUDA(cudaMemcpyAsync(ds + oXY1, hs + oXY1, total - oXY1, cudaMemcpyHostToDevice, c->stream));
     EssentialArgs& a = b.job[0];
-    a.xy1 = (const float2*)(ds + oXY1); a.xy2 = (const float2*)(ds + oXY2); a.status = status ? ds + oSt : nullptr;
-    a.E = (double*)ds; a.nsol = (int*)(ds + 8 * 90); a.inliers = (int*)(ds + 8 * 90 + 4); a.mask = ds + oMask;
-    HV_CUDA(hv_launch_essential(b, 1, c->stream));
-    c->launches += 1;
-    HV_CUDA(cudaMemcpyAsync(hs, ds, oMask + (size_t)n, cudaMemcpyDeviceToHost, c->stream));
-    HV_CUDA(cudaStreamSynchronize(c->stream));
-    memcpy(E, hs, 8 * 90);
-    memcpy(nsol, hs + 8 * 90, sizeof(int));
-    memcpy(inliers, hs + 8 * 90 + 4, sizeof(int));
-    if (n > 0) memcpy(mask, hs + oMask, (size_t)n);
-    return HV_OK;
+    HostStage s;
+    s.out(a.E, 8 * 90); s.out(a.nsol, sizeof(int)); s.out(a.inliers, sizeof(int)); s.out(a.mask, (size_t)n);
+    s.in(a.xy1, 8 * (size_t)n); s.in(a.xy2, 8 * (size_t)n); s.in(a.status, (size_t)n);
+    rc = s.send(c);
+    if (rc == HV_OK) rc = ess_run(c, b, 1);
+    return rc != HV_OK ? rc : s.recv(c);
 }
 
 int hv_find_essential_batch_device(hv_ctx* c, const hv_essential_job* jobs, int njobs, double prob, double threshold, int maxIters)
 {
     const char* who = "hv_find_essential_batch_device";
-    if (!c || !jobs) { hv_set_error("%s: NULL context or jobs", who); return HV_ERR_INVALID; }
-    if (njobs < 1 || njobs > HV_ESSENTIAL_BATCH_MAX) { hv_set_error("%s: %d jobs (1..%d per call)", who, njobs, HV_ESSENTIAL_BATCH_MAX); return HV_ERR_INVALID; }
-    int rc = ess_params(who, prob, maxIters);
+    int rc = batch_check(who, c, jobs, njobs, HV_ESSENTIAL_BATCH_MAX);
     if (rc != HV_OK) return rc;
     EssentialBatchArgs b;
-    memset(&b, 0, sizeof(b));
+    rc = ess_params(who, prob, threshold, maxIters, b);
+    if (rc != HV_OK) return rc;
     for (int j = 0; j < njobs; j++) {
         const hv_essential_job& J = jobs[j];
         char w[64];
@@ -1170,17 +1180,11 @@ int hv_find_essential_batch_device(hv_ctx* c, const hv_essential_job* jobs, int 
         rc = ess_args(w, J.d_xy1, J.d_xy2, J.d_status, J.n, J.fx, J.fy, J.cx, J.cy, J.d_E, J.d_nsol, J.d_mask, J.d_inliers, b.job[j]);
         if (rc != HV_OK) return rc;
     }
-    b.prob = prob; b.threshold = threshold; b.maxIters = maxIters;
-    HV_CUDA(cudaSetDevice(c->device));
-    rc = ess_scratch(c, b.job, njobs);
-    if (rc != HV_OK) return rc;
-    HV_CUDA(hv_launch_essential(b, njobs, c->stream));
-    c->launches += 1;
-    return HV_OK;
+    return ess_run(c, b, njobs);
 }
 
 // ------------------------------------------------------------------------------------------------ relative pose from E (N3)
-// Checks one job and fills its arguments; the intrinsics are refused as ess_args refuses them.
+// Checks one job and fills its arguments.
 static int pose_args(const char* who, const double* E, const int* nsol, const float* xy1, const float* xy2, const uint8_t* maskIn, int n,
                      double fx, double fy, double cx, double cy, double* R, double* t, uint8_t* maskOut, int* good, PoseArgs& a)
 {
@@ -1188,15 +1192,22 @@ static int pose_args(const char* who, const double* E, const int* nsol, const fl
     if (n < 0) { hv_set_error("%s: n = %d", who, n); return HV_ERR_INVALID; }
     if (n > 0 && (!xy1 || !xy2 || !maskOut)) { hv_set_error("%s: NULL xy1, xy2 or mask_out", who); return HV_ERR_INVALID; }
     if (n > HV_ESSENTIAL_MAX_POINTS) { hv_set_error("%s: %d points (at most %d)", who, n, HV_ESSENTIAL_MAX_POINTS); return HV_ERR_UNSUPPORTED; }
-    if (!std::isfinite(fx) || !std::isfinite(fy) || !std::isfinite(cx) || !std::isfinite(cy) || fx == 0.0 || fy == 0.0) {
-        hv_set_error("%s: intrinsics (%g, %g, %g, %g) not finite or a zero focal length", who, fx, fy, cx, cy);
-        return HV_ERR_UNSUPPORTED;
-    }
+    const int rc = intrinsics_check(who, fx, fy, cx, cy);
+    if (rc != HV_OK) return rc;
     memset(&a, 0, sizeof(a));
     a.E = E; a.nsol = nsol;
     a.xy1 = (const float2*)xy1; a.xy2 = (const float2*)xy2; a.maskIn = maskIn; a.n = n;
     a.fx = fx; a.fy = fy; a.cx = cx; a.cy = cy;
     a.R = R; a.t = t; a.maskOut = maskOut; a.good = good;
+    return HV_OK;
+}
+
+// the launch of b's first njobs jobs, checked (every hv_recover_pose* call)
+static int pose_run(hv_ctx* c, const PoseBatchArgs& b, int njobs)
+{
+    HV_CUDA(cudaSetDevice(c->device));
+    HV_CUDA(hv_launch_pose(b, njobs, c->stream));
+    c->launches += 1;
     return HV_OK;
 }
 
@@ -1207,13 +1218,9 @@ int hv_recover_pose_device(hv_ctx* c, const double* dE, const int* dNsol, const 
     if (!c) { hv_set_error("%s: NULL context", who); return HV_ERR_INVALID; }
     PoseBatchArgs b;
     memset(&b, 0, sizeof(b));
-    int rc = pose_args(who, dE, dNsol, dXY1, dXY2, dMaskIn, n, fx, fy, cx, cy, dR, dT, dMaskOut, dGood, b.job[0]);
-    if (rc != HV_OK) return rc;
     b.dist = dist;
-    HV_CUDA(cudaSetDevice(c->device));
-    HV_CUDA(hv_launch_pose(b, 1, c->stream));
-    c->launches += 1;
-    return HV_OK;
+    const int rc = pose_args(who, dE, dNsol, dXY1, dXY2, dMaskIn, n, fx, fy, cx, cy, dR, dT, dMaskOut, dGood, b.job[0]);
+    return rc != HV_OK ? rc : pose_run(c, b, 1);
 }
 
 int hv_recover_pose(hv_ctx* c, const double* E, const float* xy1, const float* xy2, const uint8_t* maskIn, int n, double fx, double fy,
@@ -1223,73 +1230,52 @@ int hv_recover_pose(hv_ctx* c, const double* E, const float* xy1, const float* x
     if (!c) { hv_set_error("%s: NULL context", who); return HV_ERR_INVALID; }
     PoseBatchArgs b;
     memset(&b, 0, sizeof(b));
+    b.dist = dist;
     int rc = pose_args(who, E, nullptr, xy1, xy2, maskIn, n, fx, fy, cx, cy, R, t, maskOut, good, b.job[0]);
     if (rc != HV_OK) return rc;
     for (int k = 0; k < 9; k++)
         if (!std::isfinite(E[k])) { hv_set_error("%s: E[%d] = %g is not finite", who, k, E[k]); return HV_ERR_UNSUPPORTED; }
-    b.dist = dist;
-    HV_CUDA(cudaSetDevice(c->device));
-    // staging block: [R 9 | t 3 doubles | good | mask_out n] back to the host, [E 9 doubles | xy1 8n | xy2 8n | mask_in n] to the device
-    const size_t oGood = 8 * 12, oMask = oGood + 16, oE = align_up(oMask + (size_t)n, 16), oXY1 = oE + 8 * 9;
-    const size_t oXY2 = oXY1 + 8 * (size_t)n, oMi = oXY2 + 8 * (size_t)n, total = oMi + (maskIn ? (size_t)n : 0);
-    rc = hv_ctx_reserve_stage(c, total);
-    if (rc != HV_OK) return rc;
-    uint8_t* hs = (uint8_t*)c->h_stage; uint8_t* ds = (uint8_t*)c->d_stage;
-    memcpy(hs + oE, E, 8 * 9);
-    if (n > 0) {
-        memcpy(hs + oXY1, xy1, 8 * (size_t)n);
-        memcpy(hs + oXY2, xy2, 8 * (size_t)n);
-        if (maskIn) memcpy(hs + oMi, maskIn, (size_t)n);
-    }
-    HV_CUDA(cudaMemcpyAsync(ds + oE, hs + oE, total - oE, cudaMemcpyHostToDevice, c->stream));
     PoseArgs& a = b.job[0];
-    a.E = (const double*)(ds + oE); a.xy1 = (const float2*)(ds + oXY1); a.xy2 = (const float2*)(ds + oXY2);
-    a.maskIn = maskIn ? ds + oMi : nullptr;
-    a.R = (double*)ds; a.t = (double*)(ds + 8 * 9); a.good = (int*)(ds + oGood); a.maskOut = ds + oMask;
-    HV_CUDA(hv_launch_pose(b, 1, c->stream));
-    c->launches += 1;
-    HV_CUDA(cudaMemcpyAsync(hs, ds, oMask + (size_t)n, cudaMemcpyDeviceToHost, c->stream));
-    HV_CUDA(cudaStreamSynchronize(c->stream));
-    memcpy(R, hs, 8 * 9);
-    memcpy(t, hs + 8 * 9, 8 * 3);
-    memcpy(good, hs + oGood, sizeof(int));
-    if (n > 0) memcpy(maskOut, hs + oMask, (size_t)n);
-    return HV_OK;
+    HostStage s;
+    s.out(a.R, 8 * 9); s.out(a.t, 8 * 3); s.out(a.good, sizeof(int)); s.out(a.maskOut, (size_t)n);
+    s.in(a.E, 8 * 9); s.in(a.xy1, 8 * (size_t)n); s.in(a.xy2, 8 * (size_t)n); s.in(a.maskIn, (size_t)n);
+    rc = s.send(c);
+    if (rc == HV_OK) rc = pose_run(c, b, 1);
+    return rc != HV_OK ? rc : s.recv(c);
 }
 
 int hv_recover_pose_batch_device(hv_ctx* c, const hv_pose_job* jobs, int njobs, double dist)
 {
     const char* who = "hv_recover_pose_batch_device";
-    if (!c || !jobs) { hv_set_error("%s: NULL context or jobs", who); return HV_ERR_INVALID; }
-    if (njobs < 1 || njobs > HV_ESSENTIAL_BATCH_MAX) { hv_set_error("%s: %d jobs (1..%d per call)", who, njobs, HV_ESSENTIAL_BATCH_MAX); return HV_ERR_INVALID; }
+    int rc = batch_check(who, c, jobs, njobs, HV_ESSENTIAL_BATCH_MAX);
+    if (rc != HV_OK) return rc;
     PoseBatchArgs b;
     memset(&b, 0, sizeof(b));
+    b.dist = dist;
     for (int j = 0; j < njobs; j++) {
         const hv_pose_job& J = jobs[j];
         char w[64];
         snprintf(w, sizeof(w), "%s job %d", who, j);
-        const int rc = pose_args(w, J.d_E, J.d_nsol, J.d_xy1, J.d_xy2, J.d_mask_in, J.n, J.fx, J.fy, J.cx, J.cy, J.d_R, J.d_t, J.d_mask_out,
-                                 J.d_good, b.job[j]);
+        rc = pose_args(w, J.d_E, J.d_nsol, J.d_xy1, J.d_xy2, J.d_mask_in, J.n, J.fx, J.fy, J.cx, J.cy, J.d_R, J.d_t, J.d_mask_out, J.d_good,
+                       b.job[j]);
         if (rc != HV_OK) return rc;
     }
-    b.dist = dist;
-    HV_CUDA(cudaSetDevice(c->device));
-    HV_CUDA(hv_launch_pose(b, njobs, c->stream));
-    c->launches += 1;
-    return HV_OK;
+    return pose_run(c, b, njobs);
 }
 
 // ------------------------------------------------------------------------------------------------ absolute-pose RANSAC (N3)
 // The parameters of the batch: refused as cv::solvePnPRansac 4.13 refuses them (confidence outside (0, 1), NaN included), or as the
-// device cannot run them (more than HV_PNP_MAX_ITERS iterations; iterations <= 0 runs one, as OpenCV does).
-static int pnp_params(const char* who, int iterations, double confidence)
+// device cannot run them (more than HV_PNP_MAX_ITERS iterations; iterations <= 0 runs one, as OpenCV does). Accepted, they start b.
+static int pnp_params(const char* who, int iterations, float reprojError, double confidence, PnpBatchArgs& b)
 {
     if (!(confidence > 0.0 && confidence < 1.0)) { hv_set_error("%s: confidence %g outside (0, 1)", who, confidence); return HV_ERR_INVALID; }
     if (iterations > HV_PNP_MAX_ITERS) { hv_set_error("%s: iterations %d above %d", who, iterations, HV_PNP_MAX_ITERS); return HV_ERR_UNSUPPORTED; }
+    memset(&b, 0, sizeof(b));
+    b.iterations = iterations; b.reprojError = reprojError; b.confidence = confidence;
     return HV_OK;
 }
 
-// Checks one job and fills everything but the scratch; the intrinsics are refused as ess_args refuses them.
+// Checks one job and fills everything but the scratch.
 static int pnp_args(const char* who, const float* xyz, const float* xy, const uint8_t* status, int n, double fx, double fy, double cx,
                     double cy, double* rvec, double* tvec, uint8_t* mask, int* inliers, int* ok, PnpArgs& a)
 {
@@ -1297,10 +1283,8 @@ static int pnp_args(const char* who, const float* xyz, const float* xy, const ui
     if (n < 0) { hv_set_error("%s: n = %d", who, n); return HV_ERR_INVALID; }
     if (n > 0 && (!xyz || !xy || !mask)) { hv_set_error("%s: NULL xyz, xy or mask", who); return HV_ERR_INVALID; }
     if (n > HV_PNP_MAX_POINTS) { hv_set_error("%s: %d points (at most %d)", who, n, HV_PNP_MAX_POINTS); return HV_ERR_UNSUPPORTED; }
-    if (!std::isfinite(fx) || !std::isfinite(fy) || !std::isfinite(cx) || !std::isfinite(cy) || fx == 0.0 || fy == 0.0) {
-        hv_set_error("%s: intrinsics (%g, %g, %g, %g) not finite or a zero focal length", who, fx, fy, cx, cy);
-        return HV_ERR_UNSUPPORTED;
-    }
+    const int rc = intrinsics_check(who, fx, fy, cx, cy);
+    if (rc != HV_OK) return rc;
     memset(&a, 0, sizeof(a));
     a.xyz = xyz; a.xy = (const float2*)xy; a.status = status; a.n = n;
     a.fx = fx; a.fy = fy; a.cx = cx; a.cy = cy;
@@ -1308,7 +1292,7 @@ static int pnp_args(const char* who, const float* xyz, const float* xy, const ui
     return HV_OK;
 }
 
-// points the jobs' compacted points into the context's scratch (120 bytes per point), grown as needed
+// points the jobs' compacted points into the context's scratch (120 bytes per point)
 static int pnp_scratch(hv_ctx* c, PnpArgs* jobs, int njobs)
 {
     size_t total = 0;
@@ -1319,7 +1303,7 @@ static int pnp_scratch(hv_ctx* c, PnpArgs* jobs, int njobs)
     }
     const int rc = ctx_scratch(c, total);
     if (rc != HV_OK) return rc;
-    uint8_t* p = (uint8_t*)c->d_essScratch;
+    uint8_t* p = (uint8_t*)c->d_scratch;
     for (int j = 0; j < njobs; j++) {
         const size_t n = (size_t)jobs[j].n;
         jobs[j].P = (float*)p; p += align_up(12 * n, 256);
@@ -1333,25 +1317,27 @@ static int pnp_scratch(hv_ctx* c, PnpArgs* jobs, int njobs)
     return HV_OK;
 }
 
+// the launch of b's first njobs jobs, checked (every hv_solve_pnp_ransac* call)
+static int pnp_run(hv_ctx* c, PnpBatchArgs& b, int njobs)
+{
+    HV_CUDA(cudaSetDevice(c->device));
+    const int rc = pnp_scratch(c, b.job, njobs);
+    if (rc != HV_OK) return rc;
+    HV_CUDA(hv_launch_pnp(b, njobs, c->stream));
+    c->launches += 1;
+    return HV_OK;
+}
+
 int hv_solve_pnp_ransac_device(hv_ctx* c, const float* dXYZ, const float* dXY, const uint8_t* dStatus, int n, double fx, double fy,
                                double cx, double cy, int iterations, float reprojError, double confidence, double* dRvec, double* dTvec,
                                uint8_t* dMask, int* dInliers, int* dOk)
 {
     const char* who = "hv_solve_pnp_ransac_device";
     if (!c) { hv_set_error("%s: NULL context", who); return HV_ERR_INVALID; }
-    int rc = pnp_params(who, iterations, confidence);
-    if (rc != HV_OK) return rc;
     PnpBatchArgs b;
-    memset(&b, 0, sizeof(b));
-    rc = pnp_args(who, dXYZ, dXY, dStatus, n, fx, fy, cx, cy, dRvec, dTvec, dMask, dInliers, dOk, b.job[0]);
-    if (rc != HV_OK) return rc;
-    b.iterations = iterations; b.reprojError = reprojError; b.confidence = confidence;
-    HV_CUDA(cudaSetDevice(c->device));
-    rc = pnp_scratch(c, b.job, 1);
-    if (rc != HV_OK) return rc;
-    HV_CUDA(hv_launch_pnp(b, 1, c->stream));
-    c->launches += 1;
-    return HV_OK;
+    int rc = pnp_params(who, iterations, reprojError, confidence, b);
+    if (rc == HV_OK) rc = pnp_args(who, dXYZ, dXY, dStatus, n, fx, fy, cx, cy, dRvec, dTvec, dMask, dInliers, dOk, b.job[0]);
+    return rc != HV_OK ? rc : pnp_run(c, b, 1);
 }
 
 int hv_solve_pnp_ransac(hv_ctx* c, const float* xyz, const float* xy, const uint8_t* status, int n, double fx, double fy, double cx,
@@ -1360,53 +1346,27 @@ int hv_solve_pnp_ransac(hv_ctx* c, const float* xyz, const float* xy, const uint
 {
     const char* who = "hv_solve_pnp_ransac";
     if (!c) { hv_set_error("%s: NULL context", who); return HV_ERR_INVALID; }
-    int rc = pnp_params(who, iterations, confidence);
-    if (rc != HV_OK) return rc;
     PnpBatchArgs b;
-    memset(&b, 0, sizeof(b));
-    rc = pnp_args(who, xyz, xy, status, n, fx, fy, cx, cy, rvec, tvec, mask, inliers, ok, b.job[0]);
+    int rc = pnp_params(who, iterations, reprojError, confidence, b);
+    if (rc == HV_OK) rc = pnp_args(who, xyz, xy, status, n, fx, fy, cx, cy, rvec, tvec, mask, inliers, ok, b.job[0]);
     if (rc != HV_OK) return rc;
-    b.iterations = iterations; b.reprojError = reprojError; b.confidence = confidence;
-    HV_CUDA(cudaSetDevice(c->device));
-    rc = pnp_scratch(c, b.job, 1);
-    if (rc != HV_OK) return rc;
-    // staging block: [rvec 3 | tvec 3 doubles | inliers, ok | mask n] back to the host, [xyz 12n | xy 8n (16-byte aligned: read as
-    // float2) | status n] to the device
-    const size_t oMask = 8 * 6 + 16, oXYZ = align_up(oMask + (size_t)n, 16);
-    const size_t oXY = align_up(oXYZ + 12 * (size_t)n, 16), oSt = oXY + 8 * (size_t)n, total = oSt + (status ? (size_t)n : 0);
-    rc = hv_ctx_reserve_stage(c, total);
-    if (rc != HV_OK) return rc;
-    uint8_t* hs = (uint8_t*)c->h_stage; uint8_t* ds = (uint8_t*)c->d_stage;
-    if (n > 0) {
-        memcpy(hs + oXYZ, xyz, 12 * (size_t)n);
-        memcpy(hs + oXY, xy, 8 * (size_t)n);
-        if (status) memcpy(hs + oSt, status, (size_t)n);
-    }
-    if (total > oXYZ) HV_CUDA(cudaMemcpyAsync(ds + oXYZ, hs + oXYZ, total - oXYZ, cudaMemcpyHostToDevice, c->stream));
     PnpArgs& a = b.job[0];
-    a.xyz = (const float*)(ds + oXYZ); a.xy = (const float2*)(ds + oXY); a.status = status ? ds + oSt : nullptr;
-    a.rvec = (double*)ds; a.tvec = (double*)(ds + 24); a.inliers = (int*)(ds + 48); a.ok = (int*)(ds + 52); a.mask = ds + oMask;
-    HV_CUDA(hv_launch_pnp(b, 1, c->stream));
-    c->launches += 1;
-    HV_CUDA(cudaMemcpyAsync(hs, ds, oMask + (size_t)n, cudaMemcpyDeviceToHost, c->stream));
-    HV_CUDA(cudaStreamSynchronize(c->stream));
-    memcpy(rvec, hs, 24);
-    memcpy(tvec, hs + 24, 24);
-    memcpy(inliers, hs + 48, sizeof(int));
-    memcpy(ok, hs + 52, sizeof(int));
-    if (n > 0) memcpy(mask, hs + oMask, (size_t)n);
-    return HV_OK;
+    HostStage s;
+    s.out(a.rvec, 8 * 3); s.out(a.tvec, 8 * 3); s.out(a.inliers, sizeof(int)); s.out(a.ok, sizeof(int)); s.out(a.mask, (size_t)n);
+    s.in(a.xyz, 12 * (size_t)n); s.in(a.xy, 8 * (size_t)n); s.in(a.status, (size_t)n);
+    rc = s.send(c);
+    if (rc == HV_OK) rc = pnp_run(c, b, 1);
+    return rc != HV_OK ? rc : s.recv(c);
 }
 
 int hv_solve_pnp_ransac_batch_device(hv_ctx* c, const hv_pnp_job* jobs, int njobs, int iterations, float reprojError, double confidence)
 {
     const char* who = "hv_solve_pnp_ransac_batch_device";
-    if (!c || !jobs) { hv_set_error("%s: NULL context or jobs", who); return HV_ERR_INVALID; }
-    if (njobs < 1 || njobs > HV_ESSENTIAL_BATCH_MAX) { hv_set_error("%s: %d jobs (1..%d per call)", who, njobs, HV_ESSENTIAL_BATCH_MAX); return HV_ERR_INVALID; }
-    int rc = pnp_params(who, iterations, confidence);
+    int rc = batch_check(who, c, jobs, njobs, HV_ESSENTIAL_BATCH_MAX);
     if (rc != HV_OK) return rc;
     PnpBatchArgs b;
-    memset(&b, 0, sizeof(b));
+    rc = pnp_params(who, iterations, reprojError, confidence, b);
+    if (rc != HV_OK) return rc;
     for (int j = 0; j < njobs; j++) {
         const hv_pnp_job& J = jobs[j];
         char w[64];
@@ -1415,13 +1375,7 @@ int hv_solve_pnp_ransac_batch_device(hv_ctx* c, const hv_pnp_job* jobs, int njob
                       b.job[j]);
         if (rc != HV_OK) return rc;
     }
-    b.iterations = iterations; b.reprojError = reprojError; b.confidence = confidence;
-    HV_CUDA(cudaSetDevice(c->device));
-    rc = pnp_scratch(c, b.job, njobs);
-    if (rc != HV_OK) return rc;
-    HV_CUDA(hv_launch_pnp(b, njobs, c->stream));
-    c->launches += 1;
-    return HV_OK;
+    return pnp_run(c, b, njobs);
 }
 
 // ------------------------------------------------------------------------------------------------ two-view triangulation (N3)
@@ -1447,6 +1401,15 @@ static int tri_args(const char* who, const double* P1, const double* P2, const f
     return HV_OK;
 }
 
+// the launch of b's first njobs jobs, checked (every hv_triangulate_points* call); maxn: their largest n
+static int tri_run(hv_ctx* c, const TriBatchArgs& b, int njobs, int maxn)
+{
+    HV_CUDA(cudaSetDevice(c->device));
+    HV_CUDA(hv_launch_triangulate(b, njobs, maxn, c->stream));
+    c->launches += 1;
+    return HV_OK;
+}
+
 int hv_triangulate_points_device(hv_ctx* c, const double* P1, const double* P2, const float* dXY1, const float* dXY2, const uint8_t* dStatus,
                                  const uint8_t* dStatus2, int n, float* dX4, float* dXYZ, uint8_t* dUsed)
 {
@@ -1455,11 +1418,7 @@ int hv_triangulate_points_device(hv_ctx* c, const double* P1, const double* P2, 
     TriBatchArgs b;
     memset(&b, 0, sizeof(b));
     const int rc = tri_args(who, P1, P2, dXY1, dXY2, dStatus, dStatus2, n, dX4, dXYZ, dUsed, b.job[0]);
-    if (rc != HV_OK) return rc;
-    HV_CUDA(cudaSetDevice(c->device));
-    HV_CUDA(hv_launch_triangulate(b, 1, n, c->stream));
-    c->launches += 1;
-    return HV_OK;
+    return rc != HV_OK ? rc : tri_run(c, b, 1, n);
 }
 
 int hv_triangulate_points(hv_ctx* c, const double* P1, const double* P2, const float* xy1, const float* xy2, const uint8_t* status,
@@ -1471,42 +1430,20 @@ int hv_triangulate_points(hv_ctx* c, const double* P1, const double* P2, const f
     memset(&b, 0, sizeof(b));
     int rc = tri_args(who, P1, P2, xy1, xy2, status, status2, n, X4, xyz, used, b.job[0]);
     if (rc != HV_OK) return rc;
-    HV_CUDA(cudaSetDevice(c->device));
-    // staging block: [X4 16n | xyz 12n | used n] back to the host, [xy1 8n | xy2 8n | status n | status2 n] to the device
-    const size_t N = (size_t)n;
-    const size_t oXYZ = 16 * N, oUsed = oXYZ + 12 * N, oXY1 = align_up(oUsed + N, 16), oXY2 = oXY1 + 8 * N, oSt = oXY2 + 8 * N;
-    const size_t oSt2 = oSt + (status ? N : 0), total = oSt2 + (status2 ? N : 0);
-    rc = hv_ctx_reserve_stage(c, total);
-    if (rc != HV_OK) return rc;
-    uint8_t* hs = (uint8_t*)c->h_stage; uint8_t* ds = (uint8_t*)c->d_stage;
-    if (n > 0) {
-        memcpy(hs + oXY1, xy1, 8 * N);
-        memcpy(hs + oXY2, xy2, 8 * N);
-        if (status) memcpy(hs + oSt, status, N);
-        if (status2) memcpy(hs + oSt2, status2, N);
-        HV_CUDA(cudaMemcpyAsync(ds + oXY1, hs + oXY1, total - oXY1, cudaMemcpyHostToDevice, c->stream));
-    }
     TriArgs& a = b.job[0];
-    a.xy1 = (const float2*)(ds + oXY1); a.xy2 = (const float2*)(ds + oXY2);
-    a.status = status ? ds + oSt : nullptr; a.status2 = status2 ? ds + oSt2 : nullptr;
-    a.X4 = X4 ? (float*)ds : nullptr; a.xyz = xyz ? (float*)(ds + oXYZ) : nullptr; a.used = used ? ds + oUsed : nullptr;
-    HV_CUDA(hv_launch_triangulate(b, 1, n, c->stream));
-    c->launches += 1;
-    if (n > 0) HV_CUDA(cudaMemcpyAsync(hs, ds, oUsed + N, cudaMemcpyDeviceToHost, c->stream));
-    HV_CUDA(cudaStreamSynchronize(c->stream));
-    if (n > 0) {
-        if (X4) memcpy(X4, hs, 16 * N);
-        if (xyz) memcpy(xyz, hs + oXYZ, 12 * N);
-        if (used) memcpy(used, hs + oUsed, N);
-    }
-    return HV_OK;
+    HostStage s;
+    s.out(a.X4, 16 * (size_t)n); s.out(a.xyz, 12 * (size_t)n); s.out(a.used, (size_t)n);
+    s.in(a.xy1, 8 * (size_t)n); s.in(a.xy2, 8 * (size_t)n); s.in(a.status, (size_t)n); s.in(a.status2, (size_t)n);
+    rc = s.send(c);
+    if (rc == HV_OK) rc = tri_run(c, b, 1, n);
+    return rc != HV_OK ? rc : s.recv(c);
 }
 
 int hv_triangulate_points_batch_device(hv_ctx* c, const hv_triangulate_job* jobs, int njobs)
 {
     const char* who = "hv_triangulate_points_batch_device";
-    if (!c || !jobs) { hv_set_error("%s: NULL context or jobs", who); return HV_ERR_INVALID; }
-    if (njobs < 1 || njobs > HV_ESSENTIAL_BATCH_MAX) { hv_set_error("%s: %d jobs (1..%d per call)", who, njobs, HV_ESSENTIAL_BATCH_MAX); return HV_ERR_INVALID; }
+    int rc = batch_check(who, c, jobs, njobs, HV_ESSENTIAL_BATCH_MAX);
+    if (rc != HV_OK) return rc;
     TriBatchArgs b;
     memset(&b, 0, sizeof(b));
     int maxn = 0;
@@ -1514,14 +1451,11 @@ int hv_triangulate_points_batch_device(hv_ctx* c, const hv_triangulate_job* jobs
         const hv_triangulate_job& J = jobs[j];
         char w[64];
         snprintf(w, sizeof(w), "%s job %d", who, j);
-        const int rc = tri_args(w, J.P1, J.P2, J.d_xy1, J.d_xy2, J.d_status, J.d_status2, J.n, J.d_X4, J.d_xyz, J.d_used, b.job[j]);
+        rc = tri_args(w, J.P1, J.P2, J.d_xy1, J.d_xy2, J.d_status, J.d_status2, J.n, J.d_X4, J.d_xyz, J.d_used, b.job[j]);
         if (rc != HV_OK) return rc;
         if (J.n > maxn) maxn = J.n;
     }
-    HV_CUDA(cudaSetDevice(c->device));
-    HV_CUDA(hv_launch_triangulate(b, njobs, maxn, c->stream));
-    c->launches += 1;
-    return HV_OK;
+    return tri_run(c, b, njobs, maxn);
 }
 
 // ------------------------------------------------------------------------------------------------ frame ingest (N4)

@@ -25,13 +25,12 @@ struct hv_ctx {
     HvPyrDesc* d_table = nullptr;
     std::vector<int> freeSlots;
     long long launches = 0;
-    // LK staging (host-buffer API): one pinned block + one device block, grown on demand
+    // Staging of the host-buffer calls (LK, the detectors, the two-view geometry): one pinned block + one device block, grown on demand
     void* h_stage = nullptr; void* d_stage = nullptr; size_t stageBytes = 0;
     void* hd_stage = nullptr;          // device alias of h_stage (mapped pinned memory): results are written straight to the host
-    float* d_selectScratch = nullptr; size_t selectScratchBytes = 0;     // hv_gftt_corners: key points and previous corners (device)
-    void* d_fastScratch = nullptr; size_t fastScratchBytes = 0;          // hv_fast_detect*: keypoint masks and tile counts (device)
-    void* d_gfScratch = nullptr; size_t gfScratchBytes = 0;              // hv_good_features*: per-job words, response maps, keys, grids
-    void* d_essScratch = nullptr; size_t essScratchBytes = 0;            // hv_find_essential*: per-job normalised points and indices
+    // Device scratch of the detectors and the two-view geometry (capi.cu: ctx_scratch), only ever grown. Every call carves its own regions
+    // from the start of it, so calls share it: all their launches are on `stream`, and a call's regions are dead once its last launch has run.
+    void* d_scratch = nullptr; size_t scratchBytes = 0;
     unsigned* d_done = nullptr;        // completion counter of the polled launches (device)
     unsigned doneCount = 0, seq = 0;   // host mirror of the counter / sequence number of the last polled launch
     // EKF group staging (hv_ekf_group_run_device): a call's argument blocks reach the device in one copy out of a ring of pinned blocks

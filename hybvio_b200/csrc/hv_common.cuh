@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include "../../include/hybvio_b200.h"     // the limits of the C ABI (HV_CORNER_BATCH_MAX, HV_ESSENTIAL_*, HV_PNP_*, ...)
 
 #define HV_MAX_LEVELS 6      // pyrLKMaxLevel <= 5 (HybVIO default 3, codegen/parameter_definitions.c:334-344)
 #define HV_PYR_TILE 64       // level-0 tile edge of the fused pyramid kernel; must be divisible by 2^maxLevel
@@ -99,7 +100,6 @@ cudaError_t hv_launch_gftt(const GfttArgs& a, cudaStream_t stream);
 
 // Batches of the corner step (detect, select, refine): one job per session, at most HV_CORNER_BATCH_MAX per launch. Every argument
 // block travels as a __grid_constant__ kernel parameter (at most 32764 bytes on sm_90).
-#define HV_CORNER_BATCH_MAX 64
 #define HV_KERNEL_PARAM_MAX 32764
 
 // The job of CTA b in a flattened grid: the last j with first[j] <= b, where first[] is the prefix sum of the jobs' CTA counts (a job
@@ -223,9 +223,6 @@ static_assert(sizeof(GoodFeaturesBatchArgs) <= HV_KERNEL_PARAM_MAX, "good-featur
 cudaError_t hv_launch_good_features_batch(const GoodFeaturesBatchArgs& b, int njobs, cudaStream_t stream);
 
 // ---- essential-matrix RANSAC (essential.cu): cv::findEssentialMat(..., RANSAC, prob, threshold, maxIters) on the used points
-#define HV_ESSENTIAL_BATCH_MAX 64
-#define HV_ESSENTIAL_MAX_POINTS 4096
-#define HV_ESSENTIAL_MAX_ITERS 4096
 struct EssentialArgs {
     const float2* xy1; const float2* xy2;
     const uint8_t* status;            // NULL: every point is used
@@ -263,8 +260,6 @@ static_assert(sizeof(PoseBatchArgs) <= HV_KERNEL_PARAM_MAX, "pose batch argument
 cudaError_t hv_launch_pose(const PoseBatchArgs& b, int njobs, cudaStream_t stream);     // one launch, one CTA per job
 
 // ---- absolute-pose RANSAC (pnp.cu): cv::solvePnPRansac(..., SOLVEPNP_P3P) on the used points, up to HV_ESSENTIAL_BATCH_MAX jobs
-#define HV_PNP_MAX_POINTS 4096
-#define HV_PNP_MAX_ITERS 4096
 struct PnpArgs {
     const float* xyz;                 // n x 3
     const float2* xy;
@@ -287,7 +282,6 @@ static_assert(sizeof(PnpBatchArgs) <= HV_KERNEL_PARAM_MAX, "pnp batch arguments 
 cudaError_t hv_launch_pnp(const PnpBatchArgs& b, int njobs, cudaStream_t stream);     // one launch, one CTA per job
 
 // ---- two-view triangulation (triangulate.cu): cv::triangulatePoints + convertPointsFromHomogeneous, up to HV_ESSENTIAL_BATCH_MAX jobs
-#define HV_TRIANGULATE_MAX_POINTS (1 << 20)
 struct TriArgs {
     double P1[12], P2[12];            // row-major 3 x 4
     const float2* xy1; const float2* xy2;
